@@ -376,7 +376,7 @@ int alloc_work(cs_cuboid_params &, cs_ctx *c)
     if ((rc = ensure(c, c->d_dist, px * 4))) return rc;
     if ((rc = ensure(c, c->d_mlines, nj * CS_MAXL_OUT * 7 * sizeof(double)))) return rc;
     if ((rc = ensure(c, c->d_lcounts, nj * 2 * 4))) return rc;
-    if ((rc = ensure(c, c->d_err, 16))) return rc;
+    if ((rc = ensure(c, c->d_err, 32))) return rc; /* words 0-3: the cuboid stage's flags; 4-7: the line detector's error word */
     if ((rc = ensure(c, c->d_cvalid, cand))) return rc;
     if ((rc = ensure(c, c->d_cdist, cand * 8))) return rc;
     if ((rc = ensure(c, c->d_cangle, cand * 8))) return rc;
@@ -420,7 +420,7 @@ int run_batch(cs_ctx *c, bool sync)
     cudaStream_t st = c->stream;
     c->launches = 0;
     if (c->profiling) cudaEventRecord(c->ev_total[0], st);
-    CS_CUDA(c, cudaMemsetAsync(c->d_err.p, 0, 16, st));
+    CS_CUDA(c, cudaMemsetAsync(c->d_err.p, 0, 32, st));
 
     const int n_jobs = (int)c->jobs.size(), n_objs = (int)c->objs.size();
     const uint8_t *gray = (const uint8_t *)c->d_gray.p;
@@ -439,6 +439,9 @@ int run_batch(cs_ctx *c, bool sync)
         } else if ((rc = cs_edl_run(c, (const uint8_t *)c->d_img.p, true, c->n_frames, c->w, c->h, c->stride, c->channels,
                                     c->line_prm.line_length_thres, c->online_cap, &d_lines_f32, &d_nlines)))
             return rc;
+        /* the detector's error word beside the cuboid stage's flags, so that fetch reads both with its one copy (no host sync here) */
+        const int32_t *line_err = cs_line_err_word(*(c->line_prm.use_LSD ? cs_ctx_lsd_slot(c) : cs_ctx_edl_slot(c)));
+        CS_CUDA(c, cudaMemcpyAsync((int32_t *)c->d_err.p + 4, line_err, 16, cudaMemcpyDeviceToDevice, st));
     }
     c->launches += c->line_launches - line_launches_before;
     c->d_online_counts = d_nlines;
@@ -587,9 +590,16 @@ int fetch(cs_ctx *c, cs_cuboid_rec *out, int32_t *out_counts)
     if (no == 0) return CS_OK;
     if (out) CS_CUDA(c, cudaMemcpyAsync(out, c->d_out.p, no * c->topk * sizeof(cs_cuboid_rec), cudaMemcpyDeviceToHost, c->stream));
     if (out_counts) CS_CUDA(c, cudaMemcpyAsync(out_counts, c->d_outcnt.p, no * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-    int32_t err = 0;
-    CS_CUDA(c, cudaMemcpyAsync(&err, c->d_err.p, 4, cudaMemcpyDeviceToHost, c->stream));
+    int32_t words[8] = {0, 0, 0, 0, 0, 0, 0, 0}; /* one copy: the cuboid stage's flags and the line detector's error word */
+    CS_CUDA(c, cudaMemcpyAsync(words, c->d_err.p, sizeof words, cudaMemcpyDeviceToHost, c->stream));
     CS_CUDA(c, cudaStreamSynchronize(c->stream));
+    const int32_t err = words[0], *line_err = words + 4;
+    if (c->online_lines) { /* the line detector's own word first: its overflow also shows as a segment count past online_cap (err & 4) */
+        /* a candidate overflow is not re-run here (that would need a host sync in the batch path): the batch fails; a synchronous
+         * cs_detect_lines_batch on the same context grows the buffer for later batches */
+        const int rc = c->line_prm.use_LSD ? cs_lsd_check_err(c, line_err) : cs_edl_check_err(c, line_err);
+        if (rc) return rc;
+    }
     if (err & 1) return fail(c, CS_ERR_CAPACITY, "more than %d line segments inside one ROI", CS_LINE_CAP);
     if (err & 2) return fail(c, CS_ERR_CAPACITY, "more than %d merged segments inside one ROI", CS_MAXL_OUT);
     if (err & 4) return fail(c, CS_ERR_CAPACITY, "the line detector found more than %d segments in a frame (raise max_lines_per_frame)", c->online_cap);

@@ -1452,6 +1452,7 @@ struct Buf {
     size_t cap = 0;
 };
 struct EdState {
+    CsLineHead head; /* first: the error word (cs_internal.h) */
     Buf img, tmp, blur, dx, dy, g, dir, edge, anchors, nanch, scratch, raw, nraw, out, nout, err;
     Buf rowcnt, pid, xy, flags, next, anid, redo, abits, colcnt, lgam;
     Buf segx, klx; /* key-line extras for the descriptor (cs_edl_run_keylines): per temporary slot, per kept segment */
@@ -1553,6 +1554,7 @@ static int ed_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_fra
     }
     const double logNT = 2.0 * (std::log10((double)w) + std::log10((double)h)); /* :2399, host libm like the reference */
     cudaMemsetAsync(S.edge.p, 0, px, st);
+    S.head.d_err = (int32_t *)S.err.p;
     cudaMemsetAsync(S.err.p, 0, 16, st);
     if (force_seq) { /* A/B: the round-1 kernels */
         k_ed_hblur<<<ed_grid((int64_t)px), 256, 0, st>>>(d_img, n_frames, w, h, stride, channels, (uint16_t *)S.tmp.p);
@@ -1630,13 +1632,24 @@ int cs_edl_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames
     return ed_run(c, imgs, imgs_on_device, n_frames, w, h, stride, channels, line_length_thres, cap, d_lines, d_counts, false);
 }
 
+/* the synchronous callers (the descriptor entry points, cs_lbd.cu): wait for the run and turn its error word into an error */
+static int ed_check_run(cs_ctx *c, EdState &S)
+{
+    cudaStream_t st = cs_ctx_stream(c);
+    int32_t err[4] = {0, 0, 0, 0};
+    if (cudaMemcpyAsync(err, S.err.p, sizeof err, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "EDLines error word copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return cs_edl_check_err(c, err);
+}
+
 int cs_edl_run_keylines(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int w, int h, int stride, int channels,
                         float line_length_thres, int cap, const float **d_lines, const int32_t **d_counts, const float **d_extra,
                         const int16_t **d_dx, const int16_t **d_dy)
 {
-    const int rc = ed_run(c, imgs, imgs_on_device, n_frames, w, h, stride, channels, line_length_thres, cap, d_lines, d_counts, true);
+    int rc = ed_run(c, imgs, imgs_on_device, n_frames, w, h, stride, channels, line_length_thres, cap, d_lines, d_counts, true);
     if (rc) return rc;
     EdState *S = ed_state_of(c);
+    if ((rc = ed_check_run(c, *S))) return rc;
     *d_extra = (const float *)S->klx.p;
     *d_dx = (const int16_t *)S->dx.p;
     *d_dy = (const int16_t *)S->dy.p;
@@ -1664,6 +1677,7 @@ int cs_edl_sobel_maps(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n
     if ((rc = ed_ensure(c, S.blur, px)) || (rc = ed_ensure(c, S.dx, px * 2)) || (rc = ed_ensure(c, S.dy, px * 2)) || (rc = ed_ensure(c, S.g, px * 2)) ||
         (rc = ed_ensure(c, S.dir, px)) || (rc = ed_ensure(c, S.err, 16)))
         return rc;
+    S.head.d_err = (int32_t *)S.err.p;
     cudaMemsetAsync(S.err.p, 0, 16, st);
     const dim3 g_tile((w + EDF_TW - 1) / EDF_TW, (h + EDF_TH - 1) / EDF_TH, n_frames);
     CUtensorMap tm;
@@ -1678,7 +1692,7 @@ int cs_edl_sobel_maps(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n
     S.last_frames = 0; /* the detector's debug views no longer describe these buffers */
     *d_dx = (const int16_t *)S.dx.p;
     *d_dy = (const int16_t *)S.dy.p;
-    return CS_OK;
+    return ed_check_run(c, S);
 }
 
 extern "C" int cs_debug_edlines(cs_ctx *c, int frame, uint8_t *blur, int16_t *dx, int16_t *dy, int16_t *g, uint8_t *dir, int32_t *anchors,

@@ -60,7 +60,7 @@
 #define LSD_NBINS 1024
 #define LSD_CHUNK_ROWS 8
 
-#define LSD_CAND_CAP 2048    /* candidate rectangles per frame handed from the seed loop to k_lsd_validate */
+#define LSD_CAND_CAP 2048    /* candidate rectangles per frame handed from the seed loop to k_lsd_validate, until a frame needs more */
 #define LSD_SEQ_SCAP 2048    /* region entries k_lsd_grow_seq keeps in shared memory (the rest spill to HBM; small, so that many frames share an SM) */
 #define LSD_HDR 8            /* ints of a candidate record header in the arena: n1, n2, has_line, x1 y1 x2 y2 (float bits), pad */
 
@@ -1118,7 +1118,8 @@ struct LsdGrowArgs {
     int cand_cap;
     int32_t *cand_line;  /* per candidate: {is a line, 4 floats} */
     struct LsdCandState *cand_state; /* per candidate: the state of the phase-split validation */
-    int32_t *err;        /* bit 2: more candidates in a frame than cand_cap */
+    int32_t *err;        /* [0]: 4 = more candidates in a frame than cand_cap, 8 = a TMA tile copy of k_lsd_blur did not complete;
+                          * [1]: the largest candidate count of a frame that overflowed, [2]: cand_cap */
     const double *lgam;  /* log_gamma table (cs_nfa.cuh) */
     uint32_t *ubits;     /* (W * H + 31) / 32 words per frame: the used map of k_lsd_grow_seq */
     int32_t *redo;       /* per frame: 1 = the sequential kernel must redo this frame */
@@ -1193,7 +1194,11 @@ __global__ void __launch_bounds__(32, kMinCtas) k_lsd_grow_seq(LsdGrowArgs A, in
     }
     if (lane == 0) {
         A.n_cand[f] = n_cand;
-        if (n_cand > A.cand_cap) atomicOr(A.err, 4);
+        if (n_cand > A.cand_cap) {
+            atomicOr(A.err, 4);
+            atomicMax(A.err + 1, n_cand);
+            A.err[2] = A.cand_cap;
+        }
     }
     LSD_PROF_ADD(6);
 }
@@ -1451,9 +1456,11 @@ struct Buf {
 };
 
 struct LsdState {
+    CsLineHead head; /* first: the error word (cs_internal.h) */
     Buf img, tmp, blur, scaled, modgrad, angf, pix, arena, raw, nraw, out, nout, redo, stats, lgam, ubits, cand, ncand, candline, candstate, err;
     bool lgam_filled = false;
     int last_frames = 0, last_W = 0, last_H = 0, cap = 0;
+    int cand_cap = LSD_CAND_CAP; /* candidate rectangles per frame; grown when a frame had more (lsd_grow_candidates) */
 };
 
 int ensure(cs_ctx *c, Buf &b, size_t bytes)
@@ -1505,8 +1512,8 @@ int lsd_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, i
         (rc = ensure(c, S.out, (size_t)n_frames * cap * 16)) || (rc = ensure(c, S.nout, (size_t)n_frames * 4)) ||
         (rc = ensure(c, S.redo, (size_t)n_frames * 4)) || (rc = ensure(c, S.stats, (size_t)n_frames * 16)) ||
         (rc = ensure(c, S.lgam, (size_t)CS_LGAMMA_TABLE * 8)) || (rc = ensure(c, S.ubits, (size_t)n_frames * (((size_t)W * H + 31) / 32) * 4)) ||
-        (rc = ensure(c, S.cand, (size_t)n_frames * LSD_CAND_CAP * sizeof(LsdRect))) || (rc = ensure(c, S.ncand, (size_t)n_frames * 4)) ||
-        (rc = ensure(c, S.candline, (size_t)n_frames * LSD_CAND_CAP * 20)) || (rc = ensure(c, S.candstate, (size_t)n_frames * LSD_CAND_CAP * sizeof(LsdCandState))) || (rc = ensure(c, S.err, 16)))
+        (rc = ensure(c, S.cand, (size_t)n_frames * S.cand_cap * sizeof(LsdRect))) || (rc = ensure(c, S.ncand, (size_t)n_frames * 4)) ||
+        (rc = ensure(c, S.candline, (size_t)n_frames * S.cand_cap * 20)) || (rc = ensure(c, S.candstate, (size_t)n_frames * S.cand_cap * sizeof(LsdCandState))) || (rc = ensure(c, S.err, 16)))
         return rc;
     if (!S.lgam_filled) { /* log_gamma of the integers 1 .. CS_LGAMMA_TABLE - 1, host libm like the reference */
         std::vector<double> t(CS_LGAMMA_TABLE, 0.0);
@@ -1521,7 +1528,9 @@ int lsd_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, i
     const double LOG_NT = 5 * (std::log10((double)W) + std::log10((double)H)) / 2 + std::log10(11.0);
     const int min_reg_size = (int)(-LOG_NT / std::log10(p));
 
-    cudaMemsetAsync(S.err.p, 0, 16, st);
+    int32_t *const d_err = (int32_t *)S.err.p; /* the 16-byte error word (cs_internal.h) */
+    S.head.d_err = d_err;
+    cudaMemsetAsync(d_err, 0, 16, st);
     cudaMemsetAsync(S.stats.p, 0, (size_t)n_frames * 16, st);
     const dim3 g_src((w * h + 255) / 256, n_frames), g_dst((W * H + 255) / 256, n_frames);
     if (cs_ctx_seq_lines(c)) { /* A/B: the two-pass kernels */
@@ -1533,9 +1542,9 @@ int lsd_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, i
         CUtensorMap tm;
         /* BGR frames whose rows are a multiple of 16 bytes (640 and 1280 wide are) can be staged by the copy engine */
         if (cs_ctx_use_tma(c) && channels == 3 && stride == 3 * w && cs_make_tmap_bytes(&tm, d_img, 3 * (int64_t)w, (int64_t)n_frames * h, stride, LSB_BOXW, LSB_TH + 6))
-            k_lsd_blur<true><<<g_tile, 256, 0, st>>>(tm, d_img, w, h, stride, channels, (double *)S.blur.p, (int32_t *)S.err.p);
+            k_lsd_blur<true><<<g_tile, 256, 0, st>>>(tm, d_img, w, h, stride, channels, (double *)S.blur.p, d_err);
         else
-            k_lsd_blur<false><<<g_tile, 256, 0, st>>>(tm, d_img, w, h, stride, channels, (double *)S.blur.p, (int32_t *)S.err.p);
+            k_lsd_blur<false><<<g_tile, 256, 0, st>>>(tm, d_img, w, h, stride, channels, (double *)S.blur.p, d_err);
     }
     k_lsd_resize<<<g_dst, 256, 0, st>>>((const double *)S.blur.p, n_frames, w, h, W, H, 1. / SCALE, (double *)S.scaled.p);
     k_lsd_grad<<<g_dst, 256, 0, st>>>((const double *)S.scaled.p, n_frames, W, H, rho, (double *)S.modgrad.p, (float *)S.angf.p,
@@ -1569,10 +1578,10 @@ int lsd_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, i
     A.ubits = (uint32_t *)S.ubits.p;
     A.cand = (LsdRect *)S.cand.p;
     A.n_cand = (int32_t *)S.ncand.p;
-    A.cand_cap = LSD_CAND_CAP;
+    A.cand_cap = S.cand_cap;
     A.cand_line = (int32_t *)S.candline.p;
     A.cand_state = (LsdCandState *)S.candstate.p;
-    A.err = (int32_t *)S.err.p;
+    A.err = d_err;
     A.redo = (int32_t *)S.redo.p;
     A.stats = (int32_t *)S.stats.p;
     {
@@ -1614,6 +1623,15 @@ LsdState *state_of(cs_ctx *c)
     return (LsdState *)*slot;
 }
 
+/* after a run whose error word (read back) says a frame had more candidate rectangles than the hand-off buffer held: grow the buffer to
+ * the largest count, for the next run (false: nothing to grow) */
+bool lsd_grow_candidates(LsdState &S, const int32_t err[4])
+{
+    if (!(err[0] & 4) || err[1] <= S.cand_cap) return false;
+    S.cand_cap = (err[1] + 255) & ~255;
+    return true;
+}
+
 }  // namespace
 
 /* device-to-device entry used by the online batch path: frames already in HBM, results stay in HBM */
@@ -1628,13 +1646,23 @@ int cs_lsd_run_device(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int w, int
     return CS_OK;
 }
 
-/* host frames in, results stay in HBM (the descriptor path, cs_lbd.cu) */
+/* host frames in, results stay in HBM (the synchronous descriptor path, cs_lbd.cu): waits for the run and reads its error word back; a
+ * candidate overflow grows the buffer and runs once more */
 int cs_lsd_run_host(cs_ctx *c, const uint8_t *imgs, int n_frames, int w, int h, int stride, int channels, float line_length_thres, int cap,
                     const float **d_lines, const int32_t **d_counts, const uint8_t **d_frames)
 {
     LsdState *S = state_of(c);
-    const int rc = lsd_run(c, imgs, false, n_frames, w, h, stride, channels, line_length_thres, cap, *S);
-    if (rc) return rc;
+    cudaStream_t st = cs_ctx_stream(c);
+    for (int pass = 0;; pass++) {
+        int rc = lsd_run(c, imgs, false, n_frames, w, h, stride, channels, line_length_thres, cap, *S);
+        if (rc) return rc;
+        int32_t err[4] = {0, 0, 0, 0};
+        if (cudaMemcpyAsync(err, S->err.p, sizeof err, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+            return cs_ctx_fail(c, CS_ERR_CUDA, "LSD error word copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+        if (pass == 0 && lsd_grow_candidates(*S, err)) continue;
+        if ((rc = cs_lsd_check_err(c, err))) return rc;
+        break;
+    }
     *d_lines = (const float *)S->out.p;
     *d_counts = (const int32_t *)S->nout.p;
     *d_frames = (const uint8_t *)S->img.p; /* the frames as uploaded (same stride), still in HBM */
@@ -1665,23 +1693,34 @@ int cs_detect_lines_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int widt
      * 3 octaves, tests/test_oracle_ref_octaves.py). */
     if (params->numoctaves < 1) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "numoctaves must be at least 1");
     cudaSetDevice(cs_ctx_device(c));
-    const float *d_out = nullptr;
-    const int32_t *d_nout = nullptr;
-    int rc;
-    if (params->use_LSD) {
-        LsdState *S = state_of(c);
-        rc = lsd_run(c, imgs, false, n_frames, width, height, stride, channels, params->line_length_thres, max_lines_per_frame, *S);
-        d_out = (const float *)S->out.p;
-        d_nout = (const int32_t *)S->nout.p;
-    } else
-        rc = cs_edl_run(c, imgs, false, n_frames, width, height, stride, channels, params->line_length_thres, max_lines_per_frame, &d_out, &d_nout);
-    if (rc) return rc;
     cudaStream_t st = cs_ctx_stream(c);
     std::vector<int32_t> cnt(n_frames);
-    if (cudaMemcpyAsync(cnt.data(), d_nout, (size_t)n_frames * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaMemcpyAsync(lines_xyxy, d_out, (size_t)n_frames * max_lines_per_frame * 16, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaStreamSynchronize(st) != cudaSuccess)
-        return cs_ctx_fail(c, CS_ERR_CUDA, "line result copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+    for (int pass = 0;; pass++) {
+        const float *d_out = nullptr;
+        const int32_t *d_nout = nullptr, *d_err = nullptr;
+        int rc;
+        if (params->use_LSD) {
+            LsdState *S = state_of(c);
+            rc = lsd_run(c, imgs, false, n_frames, width, height, stride, channels, params->line_length_thres, max_lines_per_frame, *S);
+            d_out = (const float *)S->out.p;
+            d_nout = (const int32_t *)S->nout.p;
+            d_err = (const int32_t *)S->err.p;
+        } else {
+            rc = cs_edl_run(c, imgs, false, n_frames, width, height, stride, channels, params->line_length_thres, max_lines_per_frame, &d_out, &d_nout);
+            d_err = cs_line_err_word(*cs_ctx_edl_slot(c));
+        }
+        if (rc) return rc;
+        int32_t err[4] = {0, 0, 0, 0};
+        if (cudaMemcpyAsync(cnt.data(), d_nout, (size_t)n_frames * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+            cudaMemcpyAsync(err, d_err, sizeof err, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+            cudaMemcpyAsync(lines_xyxy, d_out, (size_t)n_frames * max_lines_per_frame * 16, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+            cudaStreamSynchronize(st) != cudaSuccess)
+            return cs_ctx_fail(c, CS_ERR_CUDA, "line result copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+        /* a frame had more candidate rectangles than the hand-off buffer held: grow it to the batch's largest count and run once more */
+        if (params->use_LSD && pass == 0 && lsd_grow_candidates(*state_of(c), err)) continue;
+        if ((rc = params->use_LSD ? cs_lsd_check_err(c, err) : cs_edl_check_err(c, err))) return rc;
+        break;
+    }
     for (int f = 0; f < n_frames; f++) {
         if (cnt[f] > max_lines_per_frame) return cs_ctx_fail(c, CS_ERR_CAPACITY, "frame %d: %d segments exceed max_lines_per_frame", f, cnt[f]);
         n_lines[f] = cnt[f];

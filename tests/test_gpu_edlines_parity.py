@@ -109,3 +109,70 @@ def test_online_mode_with_edlines(det, oracle):
                 assert abs(float(out1[o, k]["normalized_error"]) - float(ref["cuboids"][b][k]["normalized_error"])) < 1e-9
             o += 1
     ctx.close()
+
+
+# ---- shapes, strides and the three routing regimes ----------------------------------------------------------------------------------
+
+SM_NODES = 32766   # walk-graph nodes k_ed_route keeps in shared memory (cs_edlines.cu ed_sm_nodes)
+
+
+def routing_regime(oracle, img):
+    """Which of the three routing paths a frame takes, from the oracle's gradient map: the walk graph has one node per pixel with g > 0;
+    up to SM_NODES it is walked in shared memory, up to w * h / 2 in HBM, beyond that k_ed_route_fit routes on the pixel maps."""
+    g = oracle.edl_detect(img, 15.0, want_stages=True)["stages"]["g"]
+    n = int((g > 0).sum())
+    return "shared" if n <= SM_NODES else "hbm" if n <= g.size // 2 else "pixel_map"
+
+
+@pytest.fixture(scope="module")
+def det15(det):
+    import cube_slam_b200 as cs
+    d = cs.line_lbd_detect(context=det._ctx)
+    d.line_length_thres = 15
+    return d
+
+
+def test_all_three_routing_regimes_in_one_batch(det15, oracle):
+    """A batch whose frames take the three routing paths side by side (per-frame redo flags and graph offsets), then each regime alone,
+    stage by stage; the regimes are asserted from the oracle's g map.  The 10-pixel checkerboard (pixel-map routing) has no segment."""
+    from test_oracle_ref_edlines import dense_frames
+    from test_oracle_ref_lsd import CHECKERBOARDS, checkerboard
+    frames = dense_frames()
+    board = np.repeat(checkerboard(*CHECKERBOARDS["vga_10px"])[:, :, None], 3, 2)
+    batch = np.stack([frames["checkerboard_window"], frames["room"], frames["room_noise_band"], board])
+    assert [routing_regime(oracle, img) for img in batch] == ["pixel_map", "shared", "hbm", "pixel_map"]
+    for imgs in (batch, batch[1:2], batch[2:3], batch[0:1]):
+        out = det15.detect_filter_lines_batch(imgs)
+        for f in range(len(imgs)):
+            ref = _check_frame(det15, oracle, imgs[f], f, 15.0)
+            np.testing.assert_array_equal(out[f], ref["lines"])
+    assert min(len(oracle.edl_detect(img, 15.0)["lines"]) for img in batch[:3]) >= 30
+
+
+def test_kitti_and_sxga_bgr_batches(det15, oracle):
+    """KITTI 1242 x 375 BGR (rows not a multiple of 16 bytes: byte-staged front end) and 1280 x 960 BGR (TMA-staged)."""
+    from cube_slam_b200 import synthetic as S
+    for imgs in (S.make_batch(91, 3, 1242, 375, 3, kind="kitti")[0], S.make_batch(92, 2, 1280, 960, 3)[0]):
+        out = det15.detect_filter_lines_batch(imgs)
+        for f in range(len(imgs)):
+            ref = _check_frame(det15, oracle, imgs[f], f, 15.0)
+            np.testing.assert_array_equal(out[f], ref["lines"])
+            assert len(out[f]) > 20
+
+
+@pytest.mark.parametrize("channels", [1, 3], ids=["gray", "bgr"])
+@pytest.mark.parametrize("shape", [(97, 211), (61, 64), (200, 333), (203, 241), (3, 3), (4, 5), (7, 9)],
+                         ids=lambda s: "%dx%d" % s)
+def test_odd_size_batches(det15, oracle, shape, channels):
+    """Batches of three frames at ragged sizes (test_gpu_lsd_parity.py's shape matrix); ed_run rejects frames under 8 x 8."""
+    import cube_slam_b200 as cs
+    from test_gpu_lsd_parity import odd_size_batch
+    imgs = odd_size_batch(shape[0], shape[1], channels)
+    if min(shape) < 8:
+        with pytest.raises(cs.CubeSlamError, match="INVALID_ARG"):
+            det15.detect_filter_lines_batch(imgs)
+        return
+    out = det15.detect_filter_lines_batch(imgs)
+    for f in range(len(imgs)):
+        ref = _check_frame(det15, oracle, imgs[f], f, 15.0)
+        np.testing.assert_array_equal(out[f], ref["lines"])

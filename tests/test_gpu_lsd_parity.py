@@ -20,9 +20,9 @@ def det():
     return d
 
 
-def _check_frame(det, oracle, img, frame=0):
-    ref = oracle.lsd_detect(img, 15.0, want_stages=True)
-    dbg = det.debug_frame(frame)
+def _check_frame(det, oracle, img, frame=0, cap=8192):
+    ref = oracle.lsd_detect(img, 15.0, cap=cap, want_stages=True)
+    dbg = det.debug_frame(frame, cap)
     np.testing.assert_array_equal(dbg["scaled"], ref["stages"]["scaled"])
     np.testing.assert_array_equal(dbg["modgrad"][:-1, :-1], ref["stages"]["modgrad"][:-1, :-1])
     np.testing.assert_array_equal(dbg["angles"], ref["stages"]["angles"])
@@ -132,11 +132,19 @@ def test_object_slam_sequence_parity(det, oracle, fixture_b):
 
 def test_online_batch_equals_two_calls(det, oracle):
     """cs_detect_frames_batch (lines stay on the device) == cs_detect_lines_batch followed by cs_detect_cuboids_batch."""
+    _online_equals_two_calls(det, oracle, 51, 5, 640, 480, 3, "indoor")
+
+
+def test_online_batch_equals_two_calls_at_kitti_size(det, oracle):
+    """The same at the KITTI size with 8 boxes a frame, as bench.py's c4 runs the online path."""
+    _online_equals_two_calls(det, oracle, 52, 3, 1242, 375, 8, "kitti")
+
+
+def _online_equals_two_calls(det, oracle, seed, F, w, h, n_boxes, kind):
     import cube_slam_b200 as cs
     from cube_slam_b200 import synthetic as S
-    F = 5
-    imgs, Ts, boxes, _, K = S.make_batch(51, F, 640, 480, 3, poisson=True)
-    ctx = cs.Context(0, 640, 480, F, 16, 2048)
+    imgs, Ts, boxes, _, K = S.make_batch(seed, F, w, h, n_boxes, kind=kind, poisson=(kind == "indoor"))
+    ctx = cs.Context(0, w, h, F, 16, 2048)
     ctx.set_calibration(K)
     p = cs.default_params(max_cuboid_num=2)
     lp = det.params()
@@ -235,3 +243,196 @@ def test_tma_staged_tiles_equal_byte_staged_tiles(det, oracle):
         for f in range(3):
             np.testing.assert_array_equal(got[0][f], got[256][f])
             np.testing.assert_array_equal(got[0][f], ref_fn(imgs[f], 15.0)["lines"])
+
+
+# ---- shapes, strides and densities where the kernels' indexing can go wrong ----------------------------------------------------------
+
+def test_kitti_and_sxga_bgr_batches(det, oracle):
+    """KITTI 1242 x 375 BGR (rows of 3 726 bytes, not a multiple of 16: the byte-staged blur) and 1280 x 960 BGR (the TMA-staged blur), the
+    frame shapes of bench.py's c4 and c5, stage by stage."""
+    from cube_slam_b200 import synthetic as S
+    for imgs in (S.make_batch(81, 3, 1242, 375, 3, kind="kitti")[0], S.make_batch(82, 2, 1280, 960, 3)[0]):
+        lines = det.detect_filter_lines_batch(imgs)
+        for f in range(len(imgs)):
+            ref = _check_frame(det, oracle, imgs[f], f)
+            np.testing.assert_array_equal(lines[f], ref["lines"])
+            assert len(lines[f]) > 20
+
+
+ODD_SHAPES = [(97, 211), (61, 64), (200, 333), (203, 241), (3, 3), (4, 5), (7, 9)]
+
+
+def odd_size_batch(h, w, channels):
+    """Three h x w frames: blocks of random levels (long straight edges, corners), a step edge with noise, pure noise."""
+    from test_oracle_ref_lsd import tiny_frame
+    rng = np.random.default_rng(h * 1000 + w + channels)
+    c = (channels,) if channels == 3 else ()
+    blocks = np.kron(rng.integers(0, 256, (h // 7 + 1, w // 9 + 1) + c), np.ones((7, 9) + (1,) * len(c), np.int64))[:h, :w]
+    step = tiny_frame(h, w, h + w)
+    if channels == 3:
+        step = np.stack([step, step // 2 + 40, 255 - step], 2)
+    noise = rng.integers(0, 256, (h, w) + c)
+    return np.ascontiguousarray(np.stack([blocks, step, noise]).astype(np.uint8))
+
+
+def test_odd_shapes_cover_unaligned_used_bitmaps():
+    """The 0.8-scaled frame of some of these sizes is not a whole number of 32-pixel words, so frames 1 and 2 of a batch start mid-word in
+    the seed loop's used bitmap, and its width is not a multiple of 32 (nor of the 128 pixels a seed-scan step reads)."""
+    scaled = [(int(np.rint(0.8 * h)), int(np.rint(0.8 * w))) for h, w in ODD_SHAPES]
+    assert any((H * W) % 32 for H, W in scaled) and all(W % 32 for H, W in scaled)
+
+
+@pytest.mark.parametrize("channels", [1, 3], ids=["gray", "bgr"])
+@pytest.mark.parametrize("shape", ODD_SHAPES, ids=["%dx%d" % s for s in ODD_SHAPES])
+def test_odd_size_batches(det, oracle, shape, channels):
+    imgs = odd_size_batch(shape[0], shape[1], channels)
+    lines = det.detect_filter_lines_batch(imgs)
+    for f in range(len(imgs)):
+        ref = _check_frame(det, oracle, imgs[f], f)
+        np.testing.assert_array_equal(lines[f], ref["lines"])
+
+
+def test_frames_too_small_for_lsd(det):
+    """lrint(0.8 * w) or lrint(0.8 * h) below 2: no gradient can be computed; the call fails instead of reading outside the frame."""
+    import cube_slam_b200 as cs
+    for shape in [(9, 1), (1, 9), (1, 1)]:
+        with pytest.raises(cs.CubeSlamError, match="INVALID_ARG"):
+            det.detect_filter_lines_batch(np.full((3,) + shape, 100, np.uint8))
+
+
+def test_rectangles_disc_and_ragged_noise(det, oracle):
+    """The frames tests/test_oracle_ref_lsd.py pins to the compiled reference: sharp rectangles (the reduce-radius and refine branches), a
+    blurred disc (regions cut by the density test), noise at ragged sizes and a constant frame."""
+    from test_oracle_ref_lsd import odd_and_degenerate_frames
+    for name, img in odd_and_degenerate_frames().items():
+        got = det.detect_filter_lines(img)
+        ref = _check_frame(det, oracle, img, 0)
+        np.testing.assert_array_equal(got, ref["lines"], err_msg=name)
+
+
+def detect_strided(d, imgs, pad, cap=4096):
+    """cs_detect_lines_batch on frames whose rows are `pad` bytes longer than width x channels (a cv::Mat ROI passed through the shim); the
+    padding holds bytes that must not be read."""
+    import ctypes as C
+    from cube_slam_b200 import _lib
+    F, H, W = imgs.shape[:3]
+    ch = imgs.shape[3] if imgs.ndim == 4 else 1
+    row = W * ch
+    buf = np.full((F, H, row + pad), 0xA5, np.uint8)
+    buf[:, :, :row] = imgs.reshape(F, H, row)
+    out = np.zeros((F, cap, 4), np.float32)
+    n = np.zeros(F, np.int32)
+    p = d.params()
+    rc = d._ctx.L.cs_detect_lines_batch(d._ctx.h, buf.ctypes.data, F, W, H, row + pad, ch, C.byref(p), _lib.ptr(out, C.c_float), cap,
+                                        _lib.ptr(n, C.c_int32))
+    assert rc == 0, d._ctx.L.cs_last_error(d._ctx.h).decode()
+    return [out[f, :n[f]].copy() for f in range(F)]
+
+
+def row_pads(row):
+    """a pad that keeps rows 16-byte aligned and one that breaks the alignment"""
+    aligned = (-row) % 16 or 16
+    return aligned, next(p for p in (3, 5) if (row + p) % 16)
+
+
+@pytest.mark.parametrize("use_lsd", [True, False], ids=["lsd", "edlines"])
+def test_padded_rows_equal_packed_rows(det, oracle, use_lsd):
+    import cube_slam_b200 as cs
+    from cube_slam_b200 import synthetic as S
+    d = cs.line_lbd_detect(context=det._ctx)
+    d.use_LSD = use_lsd
+    d.line_length_thres = 15
+    ref_fn = oracle.lsd_detect if use_lsd else oracle.edl_detect
+    vga = S.make_batch(84, 3, 640, 480, 3)[0]
+    for imgs in (S.make_batch(83, 3, 1242, 375, 3, kind="kitti")[0], vga, np.ascontiguousarray(vga[:, :, :, 1]), odd_size_batch(97, 211, 3)):
+        packed = d.detect_filter_lines_batch(imgs)
+        for f in range(len(imgs)):
+            np.testing.assert_array_equal(packed[f], ref_fn(imgs[f], 15.0)["lines"])
+        row = imgs.shape[2] * (imgs.shape[3] if imgs.ndim == 4 else 1)
+        for pad in row_pads(row):
+            got = detect_strided(d, imgs, pad)
+            for f in range(len(imgs)):
+                np.testing.assert_array_equal(got[f], packed[f], err_msg="row %d + pad %d, frame %d" % (row, pad, f))
+
+
+def checkerboard_batch(name):
+    """The checkerboard first, then a synthetic frame of the same size: the grown candidate buffer serves both."""
+    from cube_slam_b200 import synthetic as S
+    from test_oracle_ref_lsd import CHECKERBOARDS, checkerboard
+    w, h = CHECKERBOARDS[name][:2]
+    board = checkerboard(*CHECKERBOARDS[name])
+    if w == 1280:   # BGR: the TMA-staged blur
+        return np.stack([np.repeat(board[:, :, None], 3, 2), S.make_batch(85, 1, w, h, 3)[0][0]])
+    return np.stack([board, S.make_batch(85, 1, w, h, 3)[0][0][:, :, 1]])
+
+
+@pytest.mark.parametrize("name", ["vga_10px", "sxga_12px_noisy"])
+def test_checkerboards_beyond_the_candidate_buffer(oracle, name):
+    """More candidate rectangles in a frame than the seed loop's initial hand-off buffer holds (2 048): the synchronous entry point grows the
+    buffer and runs again.  Every raw segment is the oracle's, and the filtered matrix is the reference's (empty: no segment of a
+    checkerboard is longer than 15 pixels).  A fresh context, so that the first run overflows."""
+    import cube_slam_b200 as cs
+    d = cs.line_lbd_detect()
+    d.use_LSD = True
+    d.line_length_thres = 15
+    cap = 16384
+    imgs = checkerboard_batch(name)
+    lines = d.detect_filter_lines_batch(imgs, cap=cap)
+    for f in range(len(imgs)):
+        ref = _check_frame(d, oracle, imgs[f], f, cap)
+        np.testing.assert_array_equal(lines[f], ref["lines"])
+    assert len(d.debug_frame(0, cap)["raw_lines"]) > 2048 and lines[0].shape == (0, 4) and len(lines[1]) > 20
+    if oracle.ref_detect_filter_lines_available():
+        np.testing.assert_array_equal(lines[0], oracle.ref_detect_filter_lines(imgs[0], True, 15.0, cap=cap))
+    # again on the grown buffer, frames swapped
+    again = d.detect_filter_lines_batch(imgs[::-1].copy(), cap=cap)
+    np.testing.assert_array_equal(again[0], lines[1])
+    np.testing.assert_array_equal(again[1], lines[0])
+    d._ctx.close()
+
+
+def test_descriptor_path_on_a_checkerboard(oracle):
+    """cs_detect_descrip_lines with use_LSD on the 640 x 480 checkerboard (more than 2 048 candidate rectangles), no length filter: every
+    octave-0 key line and its descriptor."""
+    import cube_slam_b200 as cs
+    d = cs.line_lbd_detect()
+    d.use_LSD = True
+    d.line_length_thres = 15
+    img = checkerboard_batch("vga_10px")[0]
+    lines, desc = d.detect_descrip_lines(img, cap=8192, as_mat=True)
+    want = oracle.lbd_detect_keylines(img, True, -1.0)
+    assert len(lines) == len(want) > 2048
+    np.testing.assert_array_equal(lines, np.stack([want["sx"], want["sy"], want["ex"], want["ey"]], 1))
+    np.testing.assert_array_equal(desc, oracle.lbd_compute(img, want))
+    d._ctx.close()
+
+
+def test_online_path_names_the_candidate_limit(det, oracle):
+    """cs_detect_frames_batch does not add a host sync to re-run the detector: a batch with a frame of more candidate rectangles than the
+    buffer holds fails with an error that names that limit (not max_lines_per_frame).  A synchronous detector call on the same context
+    grows the buffer; the batch then runs and equals the two-call path."""
+    import cube_slam_b200 as cs
+    from cube_slam_b200 import synthetic as S
+    imgs, Ts, boxes, _, K = S.make_batch(86, 2, 640, 480, 2)
+    imgs[0] = np.repeat(checkerboard_batch("vga_10px")[0][:, :, None], 3, 2)
+    ctx = cs.Context(0, 640, 480, 2, 16, 2048)
+    ctx.set_calibration(K)
+    p = cs.default_params(max_cuboid_num=2)
+    lp = det.params()
+    assert lp.use_LSD == 1
+    with pytest.raises(cs.CubeSlamError, match="CAPACITY.*LSD candidate regions, more than the 2048 per frame"):
+        ctx.detect_frames_host(imgs, Ts, boxes, lp, p)
+    with pytest.raises(cs.CubeSlamError, match="CAPACITY.*LSD candidate regions"):   # still too small: nothing grew it
+        ctx.detect_frames_host(imgs, Ts, boxes, lp, p)
+    grow = cs.line_lbd_detect(context=ctx)
+    grow.use_LSD = True
+    grow.line_length_thres = 15
+    np.testing.assert_array_equal(grow.detect_filter_lines_batch(imgs)[0], oracle.lsd_detect(imgs[0], 15.0)["lines"])
+    out1, cnt1 = ctx.detect_frames_host(imgs, Ts, boxes, lp, p)
+    out1, cnt1 = out1.copy(), cnt1.copy()
+    lines = det.detect_filter_lines_batch(imgs)
+    np.testing.assert_array_equal(lines[0], oracle.lsd_detect(imgs[0], 15.0)["lines"])
+    out2, cnt2 = ctx.detect_batch_host(imgs, Ts, boxes, [l.astype(np.float64) for l in lines], p)
+    np.testing.assert_array_equal(cnt1, cnt2)
+    assert out1.tobytes() == out2.tobytes()
+    ctx.close()

@@ -62,3 +62,32 @@ def test_odd_sizes_and_degenerate_images(ref):
     tri[60:150, 160:240] = 120
     tri += rng.integers(0, 5, tri.shape, dtype=np.uint8)
     assert _same(ref, tri) >= 4
+
+
+def dense_frames():
+    """640 x 480 BGR frames for the three routing regimes of the GPU detector, chosen by the number of walk-graph nodes (pixels with
+    g > 0: 32 766 fit in shared memory, up to w * h / 2 = 153 600 in HBM, more go to the pixel-map kernel): a synthetic room (about 22 500
+    nodes), the same room with a band of noise over its left 120 columns (about 50 000), and a 10-pixel checkerboard with a 240 x 180 window
+    of the room (about 172 000; segments from the window only)."""
+    from cube_slam_b200 import synthetic as S
+    from test_oracle_ref_lsd import checkerboard
+    room = S.make_batch(61, 1, 640, 480, 3)[0][0]
+    noisy = room.copy()
+    noisy[:, :120] = np.random.default_rng(11).integers(0, 256, (480, 120, 3), dtype=np.uint8)
+    inset = np.repeat(checkerboard(640, 480, 10, 40, 200)[:, :, None], 3, 2)
+    inset[150:330, 200:440] = room[150:330, 200:440]
+    return {"room": room, "room_noise_band": noisy, "checkerboard_window": inset}
+
+
+def test_dense_frames_and_checkerboards(ref):
+    from test_oracle_ref_lsd import CHECKERBOARDS, checkerboard
+    for name, img in dense_frames().items():
+        assert _same(ref, img) >= 30, name
+    for name in sorted(CHECKERBOARDS):
+        _same(ref, checkerboard(*CHECKERBOARDS[name]))   # no segment: the chains break at every corner
+
+
+def test_tiny_frames(ref):
+    from test_oracle_ref_lsd import TINY_SHAPES, tiny_frame
+    for h, w in TINY_SHAPES:
+        _same(ref, tiny_frame(h, w, h * w))
