@@ -98,7 +98,7 @@ int cs_lsd_run_host(cs_ctx *c, const uint8_t *imgs, int n_frames, int w, int h, 
                     const float **d_lines, const int32_t **d_counts, const uint8_t **d_frames);
 /* The line detectors' error words: 16 bytes in HBM per workspace, cleared at the start of every run (and of cs_edl_sobel_maps), set by
  * their kernels.  LSD: [0] 4 = a frame had more candidate rectangles than the hand-off buffer holds ([1]: the largest such count, [2]: the
- * buffer's size per frame), 8 = a TMA tile copy of the blur kernel did not complete.  EDLines: [0] 1 = more anchors in a frame than
+ * buffer's size per frame), 8 = a TMA tile copy of the front end did not complete.  EDLines: [0] 1 = more anchors in a frame than
  * w * h / 5 + 1, 8 = a TMA tile copy of the front end did not complete.  The workspaces behind cs_ctx_lsd_slot / cs_ctx_edl_slot begin
  * with a CsLineHead, so the batch path finds the word without a call into the detectors.  The synchronous entry points read it back with
  * their results and fail precisely instead of returning wrong segments with CS_OK. */
@@ -108,7 +108,7 @@ struct CsLineHead {
 static inline const int32_t *cs_line_err_word(void *workspace) { return workspace ? ((const CsLineHead *)workspace)->d_err : nullptr; }
 static inline int cs_lsd_check_err(cs_ctx *c, const int32_t err[4])
 {
-    if (err[0] & 8) return cs_ctx_fail(c, CS_ERR_CUDA, "a TMA tile copy of the LSD blur kernel did not complete");
+    if (err[0] & 8) return cs_ctx_fail(c, CS_ERR_CUDA, "a TMA tile copy of the LSD front end did not complete");
     if (err[0] & 4)
         return cs_ctx_fail(c, CS_ERR_CAPACITY, "a frame has %d LSD candidate regions, more than the %d per frame the candidate buffer held", err[1], err[2]);
     return CS_OK;
