@@ -298,6 +298,17 @@ __device__ __forceinline__ bool rebuild_corners(const CsJob &jb, const CsFrame &
     return g_build_corners(jb, vps, g_top_x(jb, top_id), config_id, prm.shorted_edge_thre, c, vp1pos);
 }
 
+/* combined_score of an emitted record: the ranking key, except where the key stands in for a NaN score with +inf (NaN ranks last but is
+ * still a cuboid).  There the record reports the reference's own sum, normalized_error + skew penalty of its skew_ratio
+ * (box_proposal_detail.cpp:517-536), which is NaN when either term is. */
+__device__ __forceinline__ double g_record_score(double key, const cs_cuboid_rec &o, const cs_cuboid_params &prm)
+{
+    if (!isinf(key)) return key;
+    double skew_error = prm.weight_skew_error * g_max(o.skew_ratio - prm.nominal_skew_ratio, 0.0);
+    if (o.skew_ratio > prm.max_cut_skew) skew_error = 100;
+    return o.normalized_error + prm.weight_skew_error * skew_error;
+}
+
 extern __shared__ unsigned char fu_smem_raw[];
 
 __global__ void __launch_bounds__(FU_THREADS) k_fuse_rank(const CsObj *__restrict__ objs, const CsJob *__restrict__ jobs,
@@ -555,7 +566,7 @@ __global__ void __launch_bounds__(FU_THREADS) k_fuse_rank(const CsObj *__restric
                 o.camera_roll_delta = 0;
                 o.camera_pitch_delta = 0;
             }
-            o.combined_score = w_score[co + i];
+            o.combined_score = g_record_score(w_score[co + i], o, prm);
             o.proposal_index = raw;
             o.height_sample_id = jb.hs;
             o.valid = 1;
@@ -1045,7 +1056,7 @@ __global__ void __launch_bounds__(32 * FW_WARPS) k_fuse_warp(const CsObj *__rest
                 o.camera_roll_delta = 0;
                 o.camera_pitch_delta = 0;
             }
-            o.combined_score = w_score[co + i];
+            o.combined_score = g_record_score(w_score[co + i], o, prm);
             o.proposal_index = raw;
             o.height_sample_id = jb.hs;
             o.valid = 1;
