@@ -1658,13 +1658,15 @@ int cs_edl_run_keylines(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int
 
 /* The Sobel maps BinaryDescriptor::computeSobel builds for the descriptor (binary_descriptor.cpp:352-398, octave 0: GaussianBlur 5 x 5
  * sigma 1, then Sobel 3 x 3 into CV_16SC1) are the maps EDLineDetector::EdgeDrawing builds from OctaveKeyLines' blurred image (:811-814,
- * 1617-1622): the same front-end kernel produces them, into the EDLines workspace. */
+ * 1617-1622): the same front-end kernel produces them, into the EDLines workspace.  Any size from 1 x 1 works: the kernel reflects every
+ * tap with ed_reflect101 and masks partial tiles, and computeSobel's BORDER_REFLECT_101 maps a 1-pixel side to its one pixel.  The
+ * upper limit is the descriptor's: computeLBD clamps coordinates in a short (binary_descriptor.cpp:1184,1286-1288). */
 int cs_edl_sobel_maps(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int w, int h, int stride, int channels,
                       const int16_t **d_dx, const int16_t **d_dy)
 {
     EdState &S = *ed_state_of(c);
     cudaStream_t st = cs_ctx_stream(c);
-    if (w < 8 || h < 8 || w > 32767 || h > 32767) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "image size unsupported by the line descriptor");
+    if (w < 1 || h < 1 || w > 32767 || h > 32767) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "image size unsupported by the line descriptor");
     const size_t px = (size_t)n_frames * w * h;
     int rc;
     const uint8_t *d_img = imgs;

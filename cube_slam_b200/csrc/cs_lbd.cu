@@ -260,10 +260,10 @@ int cs_detect_descrip_lines_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, 
     const float *d_lines = nullptr, *d_extra = nullptr;
     const int32_t *d_counts = nullptr;
     const int16_t *d_dx = nullptr, *d_dy = nullptr;
+    const uint8_t *d_lsd_frames = nullptr; /* LSD: the detector's copy of the frames, for the Sobel maps once the key lines are known */
     if (params->use_LSD) {
-        const uint8_t *d_frames = nullptr;
-        if ((rc = cs_lsd_run_host(c, imgs, n_frames, width, height, stride, channels, params->line_length_thres, cap, &d_lines, &d_counts, &d_frames))) return rc;
-        if ((rc = cs_edl_sobel_maps(c, d_frames, true, n_frames, width, height, stride, channels, &d_dx, &d_dy))) return rc;
+        if ((rc = cs_lsd_run_host(c, imgs, n_frames, width, height, stride, channels, params->line_length_thres, cap, &d_lines, &d_counts, &d_lsd_frames)))
+            return rc;
     } else if ((rc = cs_edl_run_keylines(c, imgs, false, n_frames, width, height, stride, channels, params->line_length_thres, cap, &d_lines, &d_counts, &d_extra,
                                          &d_dx, &d_dy)))
         return rc;
@@ -293,6 +293,9 @@ int cs_detect_descrip_lines_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, 
             lines.push_back(L);
         }
     }
+    /* computeImpl returns before computeSobel when there is no key line (binary_descriptor.cpp:617-622), and so does this */
+    if (lines.empty()) return CS_OK;
+    if (d_lsd_frames && (rc = cs_edl_sobel_maps(c, d_lsd_frames, true, n_frames, width, height, stride, channels, &d_dx, &d_dy))) return rc;
     /* descriptors come back line after line; hand each frame's rows to its slot */
     std::vector<uint8_t> packed(lines.size() * CS_LBD_BYTES);
     if ((rc = describe(c, *state_of(c), lines, d_dx, d_dy, width, height, packed.data(), nullptr))) return rc;
