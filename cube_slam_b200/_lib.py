@@ -5,6 +5,7 @@ no CUDA device is usable, loading / cs_create fails loudly.
 """
 import ctypes as C
 import os
+import sys
 
 import numpy as np
 
@@ -58,6 +59,64 @@ KEYLINE_DTYPE = np.dtype([("start_x", "f4"), ("start_y", "f4"), ("end_x", "f4"),
                           ("response", "f4"), ("size", "f4"), ("num_pixels", "i4"), ("class_id", "i4")])
 DMATCH_DTYPE = np.dtype([("query_idx", "i4"), ("train_idx", "i4"), ("img_idx", "i4"), ("distance", "f4")])
 
+class DeviceFrames(C.Structure):
+    """cs_device_frames: n_frames x height x width x channels bytes in device memory, byte strides."""
+    _fields_ = [("data", C.c_void_p), ("n_frames", C.c_int32), ("height", C.c_int32), ("width", C.c_int32), ("channels", C.c_int32),
+                ("stride_frame", C.c_int64), ("stride_row", C.c_int64), ("stride_col", C.c_int64), ("stride_channel", C.c_int64),
+                ("channel_order", C.c_int32), ("stream", C.c_void_p)]
+
+
+ORDERS = {"bgr": 0, "rgb": 1}   # CS_ORDER_BGR, CS_ORDER_RGB
+
+
+def _stream_handle(frames, stream):
+    """cudaStream_t the producer wrote `frames` on: the given torch.cuda.Stream or raw handle; else torch's current stream for a torch tensor;
+    else the `stream` entry of __cuda_array_interface__ (1: legacy default stream, 2: per-thread default stream); else the legacy default (0)."""
+    if stream is not None:
+        return int(getattr(stream, "cuda_stream", stream))
+    torch = sys.modules.get("torch")
+    if torch is not None and isinstance(frames, torch.Tensor):
+        return int(torch.cuda.current_stream(frames.device).cuda_stream)
+    s = frames.__cuda_array_interface__.get("stream")
+    if s is None or s == 1:
+        return 0
+    return int(s)       # 2 is cudaStreamPerThread's handle; any other value is a cudaStream_t
+
+
+def device_frames(frames, order="bgr", stream=None):
+    """The cs_device_frames of `frames`, any object with __cuda_array_interface__ (a torch CUDA tensor, a CuPy array) of dtype uint8 and shape
+    (N, H, W, 3) or (N, H, W).  Strides come from the interface (None: C-contiguous).  Raises ValueError for another dtype or rank; everything
+    about the memory itself is checked by the library (cs_check_device_frames)."""
+    cai = getattr(frames, "__cuda_array_interface__", None)
+    if cai is None:
+        raise ValueError("frames must expose __cuda_array_interface__ (a CUDA tensor or array)")
+    if np.dtype(cai["typestr"]) != np.uint8:
+        raise ValueError("frames must be uint8, got %s" % cai["typestr"])
+    shape = tuple(int(v) for v in cai["shape"])
+    if len(shape) not in (3, 4):
+        raise ValueError("frames must be (N, H, W, 3) or (N, H, W), got shape %s" % (shape,))
+    strides = cai.get("strides")
+    if strides is None:
+        strides, acc = [], 1
+        for n in reversed(shape):
+            strides.insert(0, acc)
+            acc *= n
+    strides = [int(v) for v in strides]
+    d = DeviceFrames()
+    d.data = int(cai["data"][0])
+    d.n_frames, d.height, d.width = shape[:3]
+    d.channels = shape[3] if len(shape) == 4 else 1
+    d.stride_frame, d.stride_row, d.stride_col = strides[:3]
+    d.stride_channel = strides[3] if len(shape) == 4 else 0
+    if isinstance(order, str):
+        if order.lower() not in ORDERS:
+            raise ValueError("order must be 'bgr' or 'rgb', got %r" % order)
+        order = ORDERS[order.lower()]
+    d.channel_order = int(order)      # an integer goes to the library as it is
+    d.stream = _stream_handle(frames, stream) or None
+    return d
+
+
 _lib = None
 
 EXPORTS = [
@@ -70,6 +129,10 @@ EXPORTS = [
     "cs_keylines_from_lines", "cs_lbd_compute", "cs_lbd_compute_batch", "cs_detect_descrip_lines", "cs_detect_descrip_lines_batch",
     "cs_match_line_descrip", "cs_match_line_descrip_batch", "cs_lbd_debug_prepare", "cs_lbd_debug_keylines_edl", "cs_debug_last_set_pose",
 ]
+# frames already on the device (cs_ingest.cu).  They are bound where the library has them: a build of cs_context.cu alone, as the CPU test
+# suite compiles it for the host, does not; build() checks that the product library has every name of EXPORTS.
+DEVICE_FRAME_EXPORTS = ["cs_check_device_frames", "cs_batch_upload_device", "cs_batch_upload_online_device", "cs_detect_lines_batch_device"]
+EXPORTS += DEVICE_FRAME_EXPORTS
 
 
 def load():
@@ -138,7 +201,15 @@ def load():
     L.cs_lbd_debug_prepare.argtypes = [vp, i, vp, f_p, f_p]
     L.cs_lbd_debug_keylines_edl.argtypes = [f_p, f_p, i, i, i, vp]
     L.cs_debug_last_set_pose.argtypes = [u8_p, d_p, d_p, i, i, i32_p]
+    if all(hasattr(L, n) for n in DEVICE_FRAME_EXPORTS):
+        df_p = C.POINTER(DeviceFrames)
+        L.cs_check_device_frames.argtypes = [i, df_p]
+        L.cs_batch_upload_device.argtypes = [vp, df_p, d_p, d_p, i32_p, d_p, i32_p, C.POINTER(CuboidParams)]
+        L.cs_batch_upload_online_device.argtypes = [vp, df_p, d_p, d_p, i32_p, C.POINTER(LineParams), C.POINTER(CuboidParams)]
+        L.cs_detect_lines_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), f_p, C.c_int32, i32_p]
     for name in EXPORTS:
+        if name in DEVICE_FRAME_EXPORTS and not hasattr(L, name):
+            continue
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("cs_abi_version",):
             fn.restype = C.c_int

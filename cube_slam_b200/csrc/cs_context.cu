@@ -78,6 +78,7 @@ struct cs_ctx {
      * gray / Canny grids instead of queueing behind them */
     cudaStream_t stream_hi = nullptr;
     cudaEvent_t ev_mid = nullptr, ev_done = nullptr, ev_dt_fork = nullptr, ev_dt_join = nullptr;
+    cudaEvent_t ev_ingest_in = nullptr, ev_ingest_out = nullptr; /* device frames (cs_ingest.cu): producer stream -> context stream -> producer stream */
     int use_prio = 1;
     int seq_lines = 0;     /* A/B: the plain one-warp-per-frame sequential halves of the line detectors */
 
@@ -129,6 +130,14 @@ int cs_ctx_use_tma(cs_ctx *c) { return c->use_tma ? 1 : 0; }
 void **cs_ctx_edl_slot(cs_ctx *c) { return &c->edl_state; }
 void **cs_ctx_lbd_slot(cs_ctx *c) { return &c->lbd_state; }
 void cs_ctx_count_launches(cs_ctx *c, int64_t n) { c->line_launches += n; }
+void cs_ctx_ingest_events(cs_ctx *c, cudaEvent_t *in, cudaEvent_t *out)
+{
+    *in = c->ev_ingest_in;
+    *out = c->ev_ingest_out;
+}
+/* the message of the calling thread's last failed cs_check_device_frames (no context to hold it); cs_last_error(NULL) returns it */
+static thread_local std::string t_frames_err;
+void cs_set_frames_error(const char *msg) { t_frames_err = msg ? msg : ""; }
 int cs_ctx_fail(cs_ctx *c, int code, const char *fmt, ...)
 {
     char buf[512];
@@ -527,8 +536,9 @@ int run_batch(cs_ctx *c, bool sync)
 
 int store_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels, const double *T_wc,
                 const double *boxes, const int32_t *box_offsets, const double *lines, const int32_t *line_offsets,
-                const cs_cuboid_params *params, const cs_line_params *online = nullptr)
+                const cs_cuboid_params *params, const cs_line_params *online = nullptr, bool device_frames = false)
 {
+    /* device_frames: imgs is unused and the batch is left unprepared; the caller fills d_img (cs_ingest.cu) and then marks it prepared */
     std::vector<int32_t> zero_off;
     if (online) { /* no input lines: CSR of zeros */
         zero_off.assign((size_t)std::max(n_frames, 0) + 1, 0);
@@ -536,7 +546,7 @@ int store_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int width, int hei
         lines = nullptr;
     }
     if (!c) return CS_ERR_INVALID_ARG;
-    if (!imgs || n_frames <= 0 || width <= 0 || height <= 0 || !T_wc || !box_offsets || !line_offsets || !params)
+    if ((!imgs && !device_frames) || n_frames <= 0 || width <= 0 || height <= 0 || !T_wc || !box_offsets || !line_offsets || !params)
         return fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
     if (channels != 1 && channels != 3) return fail(c, CS_ERR_INVALID_ARG, "channels must be 1 or 3");
     if (stride < width * channels) return fail(c, CS_ERR_INVALID_ARG, "stride smaller than a row");
@@ -577,8 +587,9 @@ int store_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int width, int hei
     if ((rc = ensure(c, c->d_img, img_bytes + 64))) return rc;
     if ((rc = ensure(c, c->d_gray, (size_t)n_frames * height * width + 64))) return rc;
     if ((rc = ensure(c, c->d_lines, std::max<size_t>((size_t)nl * 4 * sizeof(double), 64)))) return rc;
-    CS_CUDA(c, cudaMemcpyAsync(c->d_img.p, imgs, img_bytes, cudaMemcpyHostToDevice, c->stream));
+    if (!device_frames) CS_CUDA(c, cudaMemcpyAsync(c->d_img.p, imgs, img_bytes, cudaMemcpyHostToDevice, c->stream));
     if (nl) CS_CUDA(c, cudaMemcpyAsync(c->d_lines.p, lines, (size_t)nl * 4 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    if (device_frames) return prepare_tables(c);
     c->prepared = true;
     return prepare_tables(c);
 }
@@ -709,6 +720,20 @@ int detect_batch_carried(cs_ctx *c, const uint8_t *imgs, int n_frames, int width
 
 }  // namespace
 
+/* cs_batch_upload[_online]_device (cs_ingest.cu): everything of the host forms but the frames, which the caller copies into *d_img (packed
+ * rows, pitch width * channels) on the context stream and then marks the batch prepared */
+int cs_ctx_store_device_batch(cs_ctx *c, int n_frames, int width, int height, int channels, const double *T_wc, const double *boxes,
+                              const int32_t *box_offsets, const double *lines, const int32_t *line_offsets, const cs_cuboid_params *params,
+                              const cs_line_params *online, uint8_t **d_img)
+{
+    const int rc = store_batch(c, nullptr, n_frames, width, height, width * channels, channels, T_wc, boxes, box_offsets, lines, line_offsets, params,
+                               online, true);
+    if (rc) return rc;
+    *d_img = (uint8_t *)c->d_img.p;
+    return CS_OK;
+}
+void cs_ctx_mark_prepared(cs_ctx *c) { c->prepared = true; }
+
 /* ============================================================================================ C ABI */
 extern "C" {
 
@@ -783,6 +808,8 @@ cs_ctx *cs_create(int device, int max_width, int max_height, int max_frames, int
     cudaEventCreateWithFlags(&c->ev_done, cudaEventDisableTiming);
     cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
     cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming);
+    cudaEventCreateWithFlags(&c->ev_ingest_in, cudaEventDisableTiming);
+    cudaEventCreateWithFlags(&c->ev_ingest_out, cudaEventDisableTiming);
     for (int s = 0; s <= ST_COUNT; s++) cudaEventCreate(&c->ev[s]);
     cudaEventCreate(&c->ev_total[0]);
     cudaEventCreate(&c->ev_total[1]);
@@ -811,6 +838,8 @@ void cs_destroy(cs_ctx *c)
     cudaEventDestroy(c->ev_total[1]);
     cudaEventDestroy(c->ev_fork);
     cudaEventDestroy(c->ev_join);
+    cudaEventDestroy(c->ev_ingest_in);
+    cudaEventDestroy(c->ev_ingest_out);
     cudaStreamDestroy(c->stream2);
     cudaStreamDestroy(c->stream_hi);
     if (c->gather_stream) cudaStreamDestroy(c->gather_stream);
@@ -824,7 +853,11 @@ void cs_destroy(cs_ctx *c)
     delete c;
 }
 
-const char *cs_last_error(const cs_ctx *c) { return c ? c->err.c_str() : "null context (cs_create failed: no CUDA device?)"; }
+const char *cs_last_error(const cs_ctx *c)
+{
+    if (c) return c->err.c_str();
+    return t_frames_err.empty() ? "null context (cs_create failed: no CUDA device?)" : t_frames_err.c_str();
+}
 
 int cs_set_calibration(cs_ctx *c, const double K[9])
 {

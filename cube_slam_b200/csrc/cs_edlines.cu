@@ -1626,6 +1626,12 @@ static int ed_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_fra
     return CS_OK;
 }
 
+uint8_t *cs_edl_frame_buffer(cs_ctx *c, size_t bytes)
+{
+    EdState &S = *ed_state_of(c);
+    return ed_ensure(c, S.img, bytes) ? nullptr : (uint8_t *)S.img.p;
+}
+
 int cs_edl_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int w, int h, int stride, int channels, float line_length_thres,
                int cap, const float **d_lines, const int32_t **d_counts)
 {

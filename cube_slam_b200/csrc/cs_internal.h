@@ -120,6 +120,19 @@ static inline int cs_edl_check_err(cs_ctx *c, const int32_t err[4])
     return CS_OK;
 }
 void **cs_ctx_lbd_slot(cs_ctx *c);          /* owned by cs_lbd.cu */
+
+/* frames already on the device (cs_ingest.cu) */
+int cs_ctx_store_device_batch(cs_ctx *c, int n_frames, int width, int height, int channels, const double *T_wc, const double *boxes,
+                              const int32_t *box_offsets, const double *lines, const int32_t *line_offsets, const cs_cuboid_params *params,
+                              const cs_line_params *online, uint8_t **d_img);
+void cs_ctx_mark_prepared(cs_ctx *c);
+void cs_set_frames_error(const char *msg);  /* what cs_last_error(NULL) reports after a failed cs_check_device_frames */
+/* the line detectors' own frame buffers (the ones cs_detect_lines_batch copies host frames into), grown to `bytes`; null on failure */
+uint8_t *cs_lsd_frame_buffer(cs_ctx *c, size_t bytes);
+uint8_t *cs_edl_frame_buffer(cs_ctx *c, size_t bytes);
+/* the body of cs_detect_lines_batch after its argument checks, on host frames or on frames already on the device */
+int cs_detect_lines_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int width, int height, int stride, int channels,
+                        const cs_line_params *params, float *lines_xyxy, int32_t max_lines_per_frame, int32_t *n_lines);
 void cs_lbd_destroy(void *state);           /* called from cs_destroy */
 
 #endif

@@ -1679,20 +1679,15 @@ void cs_lsd_destroy(void *state)
     delete S;
 }
 
-extern "C" {
-
-int cs_detect_lines_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
-                          const cs_line_params *params, float *lines_xyxy, int32_t max_lines_per_frame, int32_t *n_lines)
+uint8_t *cs_lsd_frame_buffer(cs_ctx *c, size_t bytes)
 {
-    if (!c) return CS_ERR_INVALID_ARG;
-    if (!imgs || !params || !lines_xyxy || !n_lines || n_frames <= 0 || width <= 0 || height <= 0 || max_lines_per_frame <= 0)
-        return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
-    if (channels != 1 && channels != 3) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "channels must be 1 or 3"); /* LSDDetector.cpp:163-164 throws on depth != 0 */
-    if (stride < width * channels) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "stride smaller than a row");
-    /* More octaves change nothing here: filter_lines keeps octave 0 only (line_lbd_allclass.cpp:200-207) and octave 0 is detected first and
-     * independently of the others in both detectors, so the matrix is the one-octave one (checked against the compiled reference with 2 and
-     * 3 octaves, tests/test_oracle_ref_octaves.py). */
-    if (params->numoctaves < 1) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "numoctaves must be at least 1");
+    LsdState *S = state_of(c);
+    return ensure(c, S->img, bytes) ? nullptr : (uint8_t *)S->img.p;
+}
+
+int cs_detect_lines_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int width, int height, int stride, int channels,
+                        const cs_line_params *params, float *lines_xyxy, int32_t max_lines_per_frame, int32_t *n_lines)
+{
     cudaSetDevice(cs_ctx_device(c));
     cudaStream_t st = cs_ctx_stream(c);
     std::vector<int32_t> cnt(n_frames);
@@ -1702,12 +1697,13 @@ int cs_detect_lines_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int widt
         int rc;
         if (params->use_LSD) {
             LsdState *S = state_of(c);
-            rc = lsd_run(c, imgs, false, n_frames, width, height, stride, channels, params->line_length_thres, max_lines_per_frame, *S);
+            rc = lsd_run(c, imgs, imgs_on_device, n_frames, width, height, stride, channels, params->line_length_thres, max_lines_per_frame, *S);
             d_out = (const float *)S->out.p;
             d_nout = (const int32_t *)S->nout.p;
             d_err = (const int32_t *)S->err.p;
         } else {
-            rc = cs_edl_run(c, imgs, false, n_frames, width, height, stride, channels, params->line_length_thres, max_lines_per_frame, &d_out, &d_nout);
+            rc = cs_edl_run(c, imgs, imgs_on_device, n_frames, width, height, stride, channels, params->line_length_thres, max_lines_per_frame, &d_out,
+                            &d_nout);
             d_err = cs_line_err_word(*cs_ctx_edl_slot(c));
         }
         if (rc) return rc;
@@ -1727,6 +1723,23 @@ int cs_detect_lines_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int widt
         n_lines[f] = cnt[f];
     }
     return CS_OK;
+}
+
+extern "C" {
+
+int cs_detect_lines_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
+                          const cs_line_params *params, float *lines_xyxy, int32_t max_lines_per_frame, int32_t *n_lines)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    if (!imgs || !params || !lines_xyxy || !n_lines || n_frames <= 0 || width <= 0 || height <= 0 || max_lines_per_frame <= 0)
+        return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
+    if (channels != 1 && channels != 3) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "channels must be 1 or 3"); /* LSDDetector.cpp:163-164 throws on depth != 0 */
+    if (stride < width * channels) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "stride smaller than a row");
+    /* More octaves change nothing here: filter_lines keeps octave 0 only (line_lbd_allclass.cpp:200-207) and octave 0 is detected first and
+     * independently of the others in both detectors, so the matrix is the one-octave one (checked against the compiled reference with 2 and
+     * 3 octaves, tests/test_oracle_ref_octaves.py). */
+    if (params->numoctaves < 1) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "numoctaves must be at least 1");
+    return cs_detect_lines_run(c, imgs, false, n_frames, width, height, stride, channels, params, lines_xyxy, max_lines_per_frame, n_lines);
 }
 
 int cs_detect_lines(cs_ctx *c, const uint8_t *img, int width, int height, int stride, int channels, const cs_line_params *params,

@@ -83,6 +83,11 @@ class Context(object):
             ch = 1
         else:
             F, H, W, ch = imgs.shape
+        Ts, boxes, box_off, lines, line_off = Context._pack_tables(F, Ts, boxes_list, lines_list)
+        return imgs, F, H, W, ch, Ts, boxes, box_off, lines, line_off
+
+    @staticmethod
+    def _pack_tables(F, Ts, boxes_list, lines_list):
         Ts = np.ascontiguousarray(Ts, np.float64).reshape(F, 16)
         box_off = np.zeros(F + 1, np.int32)
         line_off = np.zeros(F + 1, np.int32)
@@ -100,7 +105,7 @@ class Context(object):
             boxes = np.zeros((1, 5))
         if len(lines) == 0:
             lines = np.zeros((1, 4))
-        return imgs, F, H, W, ch, Ts, boxes, box_off, lines, line_off
+        return Ts, boxes, box_off, lines, line_off
 
     def set_calibration(self, K):
         K = np.ascontiguousarray(K, np.float64).reshape(9)
@@ -124,6 +129,32 @@ class Context(object):
         self._box_off = box_off
         self.check(self.L.cs_batch_upload_online(self.h, imgs.ctypes.data, F, W, H, W * ch, ch, _lib.ptr(Ts, C.c_double),
                                                  _lib.ptr(boxes, C.c_double), _lib.ptr(box_off, C.c_int32), C.byref(line_params), C.byref(params)))
+
+    def upload_device(self, frames, Ts, boxes_list, lines_list, params, order="bgr", stream=None):
+        """cs_batch_upload_device: upload() with frames already on the GPU -- any object with __cuda_array_interface__ (a torch CUDA tensor, a
+        CuPy array), uint8, (N, H, W, 3) or (N, H, W), any strides.  order: "bgr" or "rgb".  stream: the stream the frames were written on
+        (torch.cuda.Stream or raw handle; default: torch's current stream for a torch tensor, else the interface's, else the legacy default
+        stream).  Returns without blocking the host; work queued on that stream afterwards waits until the library has read the frames."""
+        fr = _lib.device_frames(frames, order, stream)
+        F = fr.n_frames
+        Ts, boxes, box_off, lines, line_off = self._pack_tables(F, Ts, boxes_list, lines_list)
+        self._n_obj = int(box_off[-1])
+        self._topk = int(params.max_cuboid_num)
+        self._box_off = box_off
+        self.check(self.L.cs_batch_upload_device(self.h, C.byref(fr), _lib.ptr(Ts, C.c_double), _lib.ptr(boxes, C.c_double),
+                                                 _lib.ptr(box_off, C.c_int32), _lib.ptr(lines, C.c_double), _lib.ptr(line_off, C.c_int32),
+                                                 C.byref(params)))
+
+    def upload_online_device(self, frames, Ts, boxes_list, line_params, params, order="bgr", stream=None):
+        """cs_batch_upload_online_device: upload_online() with frames already on the GPU (see upload_device)."""
+        fr = _lib.device_frames(frames, order, stream)
+        F = fr.n_frames
+        Ts, boxes, box_off, _, _ = self._pack_tables(F, Ts, boxes_list, [np.zeros((0, 4))] * F)
+        self._n_obj = int(box_off[-1])
+        self._topk = int(params.max_cuboid_num)
+        self._box_off = box_off
+        self.check(self.L.cs_batch_upload_online_device(self.h, C.byref(fr), _lib.ptr(Ts, C.c_double), _lib.ptr(boxes, C.c_double),
+                                                        _lib.ptr(box_off, C.c_int32), C.byref(line_params), C.byref(params)))
 
     def detect_frames_host(self, imgs, Ts, boxes_list, line_params, params, out=None, counts=None):
         """cs_detect_frames_batch: detect_filter_lines + detect_cuboid per frame, host buffers in / out."""

@@ -49,6 +49,19 @@ class line_lbd_detect(object):
             raise CubeSlamError("%s: %s" % (_lib.STATUS_NAMES.get(rc, rc), self._ctx.L.cs_last_error(self._ctx.h).decode()))
         return [out[f, :n[f]].copy() for f in range(F)]
 
+    def detect_filter_lines_device(self, frames, order="bgr", cap=4096, stream=None):
+        """detect_filter_lines_batch on frames already on the GPU: any object with __cuda_array_interface__ (a torch CUDA tensor, a CuPy array),
+        uint8, (N, H, W, 3) or (N, H, W), any strides; order "bgr" or "rgb"; stream as Context.upload_device.  The frames go to the
+        detector's own buffer, so a batch uploaded to the same context keeps its frames."""
+        fr = _lib.device_frames(frames, order, stream)
+        F = fr.n_frames
+        out = np.zeros((F, cap, 4), np.float32)
+        n = np.zeros(F, np.int32)
+        p = self.params()
+        self._ctx.check(self._ctx.L.cs_detect_lines_batch_device(self._ctx.h, C.byref(fr), C.byref(p), _lib.ptr(out, C.c_float), cap,
+                                                                  _lib.ptr(n, C.c_int32)))
+        return [out[f, :n[f]].copy() for f in range(F)]
+
     def detect_raw_lines(self, gray_img, downsample_img=False, cap=8192):
         """detect_raw_lines(gray_img, lines_mat, downsample_img) (line_lbd_allclass.cpp:174-189): every octave-0 segment, no length filter ->
         n x 4 float32; with downsample_img the image is halved first (cv::resize, as the reference does) and the lines scaled by 2."""

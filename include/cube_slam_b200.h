@@ -173,6 +173,41 @@ int cs_batch_upload(cs_ctx *ctx, const uint8_t *imgs, int n_frames, int width, i
 int cs_batch_upload_online(cs_ctx *ctx, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
                            const double *T_wc, const double *boxes, const int32_t *box_offsets,
                            const cs_line_params *line_params, const cs_cuboid_params *params);
+
+/* ---- frames already in GPU memory ---------------------------------------------------------------------------------------------------- */
+/* A batch of frames that lives on the device, described as n_frames x height x width x channels bytes with byte strides, so that any strided
+ * view is one descriptor: packed NHWC, planar NCHW (a permute(0, 2, 3, 1) view), a crop (a slice), every other frame (t[::2]), the first
+ * three channels of BGRA / RGBA (t[..., :3]).  channels 3 is BGR or RGB (channel_order), channels 1 is gray.  The library copies the view
+ * into its own packed buffer (pitch width * channels, BGR or gray) on the device -- one device-to-device copy when the view is already
+ * packed BGR or gray, else the kernel k_ingest_frames -- and everything after that is the host path's code.
+ * Stream order both ways, without a host block: the copy waits for the work queued on `stream` before the call, and work queued on `stream`
+ * after the call (overwriting or freeing the frames) waits for the copy. */
+#define CS_ORDER_BGR 0
+#define CS_ORDER_RGB 1
+typedef struct cs_device_frames {
+    const uint8_t *data;                     /* device (or managed) memory on the context's device: byte (0, 0, 0, 0) of the view */
+    int32_t n_frames, height, width, channels; /* channels 1 or 3 */
+    int64_t stride_frame, stride_row, stride_col, stride_channel; /* bytes, >= 0 (stride_channel is ignored when channels == 1) */
+    int32_t channel_order;                   /* CS_ORDER_BGR or CS_ORDER_RGB; ignored when channels == 1 */
+    void *stream;                            /* cudaStream_t the producer wrote the frames on; NULL = the legacy default stream */
+} cs_device_frames;
+
+/* Host-only check of a descriptor, made by the three calls below before they enqueue anything: CS_ERR_INVALID_ARG when the pointer is not
+ * device or managed memory on `device`, a stride is negative, channels is not 1 or 3, the order is unknown, or the last byte the view
+ * touches lies outside the pointer's allocation.  The text of a failure is what cs_last_error(NULL) returns on the calling thread. */
+int cs_check_device_frames(int device, const cs_device_frames *frames);
+/* cs_batch_upload / cs_batch_upload_online with the frames taken from the device.  Poses, boxes and lines stay host buffers, as in the
+ * host forms.  Returns once the copy is enqueued on the context stream; cs_batch_run[_async], cs_batch_fetch, cs_batch_device_records and
+ * cs_allgather_topk then work as after the host forms. */
+int cs_batch_upload_device(cs_ctx *ctx, const cs_device_frames *frames, const double *T_wc, const double *boxes, const int32_t *box_offsets,
+                           const double *lines, const int32_t *line_offsets, const cs_cuboid_params *params);
+int cs_batch_upload_online_device(cs_ctx *ctx, const cs_device_frames *frames, const double *T_wc, const double *boxes,
+                                  const int32_t *box_offsets, const cs_line_params *line_params, const cs_cuboid_params *params);
+/* cs_detect_lines_batch on device frames.  The frames go to the line detector's own buffer, as the host form's do, never to the one a batch
+ * uploaded to the context reads from.  Synchronous, like the host form. */
+int cs_detect_lines_batch_device(cs_ctx *ctx, const cs_device_frames *frames, const cs_line_params *params, float *lines_xyxy,
+                                 int32_t max_lines_per_frame, int32_t *n_lines /* n_frames */);
+
 int cs_batch_run(cs_ctx *ctx);                       /* host-side sampling tables + every kernel; synchronous */
 int cs_batch_run_async(cs_ctx *ctx);                 /* same, returns after enqueueing on the context stream */
 int cs_batch_fetch(cs_ctx *ctx, cs_cuboid_rec *out, int32_t *out_counts);
