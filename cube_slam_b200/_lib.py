@@ -133,6 +133,9 @@ EXPORTS = [
 # suite compiles it for the host, does not; build() checks that the product library has every name of EXPORTS.
 DEVICE_FRAME_EXPORTS = ["cs_check_device_frames", "cs_batch_upload_device", "cs_batch_upload_online_device", "cs_detect_lines_batch_device"]
 EXPORTS += DEVICE_FRAME_EXPORTS
+# k-nearest-neighbour and radius matching of line descriptors (cs_lbd.cu), bound the same way
+MATCHER_EXPORTS = ["cs_knn_match_line_descrip", "cs_knn_match_line_descrip_batch", "cs_radius_match_line_descrip", "cs_radius_match_line_descrip_batch"]
+EXPORTS += MATCHER_EXPORTS
 
 
 def load():
@@ -198,6 +201,12 @@ def load():
     L.cs_detect_descrip_lines_batch.argtypes = [vp, vp, i, i, i, i, i, C.POINTER(LineParams), vp, u8_p, C.c_int32, i32_p]
     L.cs_match_line_descrip.argtypes = [vp, u8_p, i, u8_p, i, C.c_float, vp, i32_p]
     L.cs_match_line_descrip_batch.argtypes = [vp, u8_p, i32_p, u8_p, i32_p, i, C.c_float, vp, i32_p]
+    i64_p = C.POINTER(C.c_int64)
+    if all(hasattr(L, n) for n in MATCHER_EXPORTS):
+        L.cs_knn_match_line_descrip.argtypes = [vp, u8_p, i, u8_p, i, i, u8_p, vp, i32_p]
+        L.cs_knn_match_line_descrip_batch.argtypes = [vp, u8_p, i32_p, u8_p, i32_p, i, i, u8_p, vp, i32_p]
+        L.cs_radius_match_line_descrip.argtypes = [vp, u8_p, i, u8_p, i, C.c_float, u8_p, vp, C.c_int64, i64_p]
+        L.cs_radius_match_line_descrip_batch.argtypes = [vp, u8_p, i32_p, u8_p, i32_p, i, C.c_float, u8_p, vp, C.c_int64, i64_p]
     L.cs_lbd_debug_prepare.argtypes = [vp, i, vp, f_p, f_p]
     L.cs_lbd_debug_keylines_edl.argtypes = [f_p, f_p, i, i, i, vp]
     L.cs_debug_last_set_pose.argtypes = [u8_p, d_p, d_p, i, i, i32_p]
@@ -208,7 +217,7 @@ def load():
         L.cs_batch_upload_online_device.argtypes = [vp, df_p, d_p, d_p, i32_p, C.POINTER(LineParams), C.POINTER(CuboidParams)]
         L.cs_detect_lines_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), f_p, C.c_int32, i32_p]
     for name in EXPORTS:
-        if name in DEVICE_FRAME_EXPORTS and not hasattr(L, name):
+        if name in DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS and not hasattr(L, name):
             continue
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("cs_abi_version",):

@@ -5,6 +5,7 @@
  *            line_lbd/libs/binary_descriptor.cpp:352-416,587-790,1146-1509   computeSobel, binaryConversion, compute / computeImpl, computeLBD
  *            line_lbd/libs/LSDDetector.cpp:226-250                           the KeyLine fields of the LSD flavour (host)
  *            line_lbd/libs/binary_descriptor_matcher.cpp:196-262,598-756     BinaryDescriptorMatcher::match, Mihasher::batchquery / query
+ *            line_lbd/libs/binary_descriptor_matcher.cpp:264-341,431-507     BinaryDescriptorMatcher::knnMatch, radiusMatch (pairwise forms)
  *
  *   k_lbd_describe   one 64-thread CTA per key line.  Thread hID walks row hID of the 63-row support region along the line (one int16
  *                    gather from each Sobel map per step, float sums in the reference's order); after a barrier 72 threads add the rows
@@ -17,6 +18,9 @@
  *   k_lbd_match      one 128-thread CTA per query descriptor: every thread takes train codes 128 apart, two 16-byte loads each, builds the
  *                    64-bit key (distance, radius, substring, pattern, train index) that reproduces the multi-index hash's visiting order
  *                    and the CTA reduces to the minimum.  32 bytes per (query, train) pair, all of it in L2 for a frame pair.
+ *   k_lbd_knn2       knnMatch with k <= 2: k_lbd_match's shape keeping the two smallest keys per thread, merged by shuffles.
+ *   k_lbd_match_sorted   knnMatch with k > 2 and radiusMatch: one 256-thread CTA per query counts the keys it keeps, stages them in shared
+ *                    memory at a CTA-wide prefix and sorts them (bitonic); radius calls it twice (counts, then keys at host offsets).
  *   The Sobel maps come from the EDLines front-end kernel (cs_edlines.cu: k_ed_front), which is what computeSobel computes.
  *
  * Host side: cos / sin of the line direction, the mid point and the Gaussian weights are computed here with libm exactly as the reference
@@ -43,6 +47,7 @@ struct Buf {
 };
 struct LbdState {
     Buf lines, desc, fdesc, coef, q, t, pairq, toff, keys;
+    Buf mkeys, moff, mcnt; /* knn / radius matching: sorted keys, their per-query offsets and counts */
     bool coef_filled = false;
 };
 
@@ -179,12 +184,79 @@ int check_image_args(cs_ctx *c, const void *imgs, int n_frames, int width, int h
     return CS_OK;
 }
 
+/* the pair CSRs of the knn / radius calls: start at 0, do not decrease, every train set within the shared-memory bound */
+int check_pairs(cs_ctx *c, const int32_t *qo, const int32_t *to, int n_pairs)
+{
+    if (n_pairs <= 0 || !qo || !to) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
+    if (qo[0] != 0 || to[0] != 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "offsets must start at 0");
+    for (int p = 0; p < n_pairs; p++) {
+        if (qo[p + 1] < qo[p] || to[p + 1] < to[p]) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "offsets must not decrease");
+        if (to[p + 1] - to[p] > CS_LBD_KNN_MAX_TRAIN)
+            return cs_ctx_fail(c, CS_ERR_CAPACITY, "pair %d has %d train codes: knn / radius matching takes at most %d per pair", p, to[p + 1] - to[p],
+                               CS_LBD_KNN_MAX_TRAIN);
+    }
+    return CS_OK;
+}
+
+/* codes of every pair to the device (S.q, S.t), with the pair of each query (S.pairq, and on the host in pair_of) and the train CSR (S.toff) */
+int upload_pairs(cs_ctx *c, LbdState &S, const uint8_t *query32, const int32_t *qo, const uint8_t *train32, const int32_t *to, int n_pairs,
+                 std::vector<int32_t> &pair_of)
+{
+    const int nq = qo[n_pairs], nt = to[n_pairs];
+    cudaStream_t st = cs_ctx_stream(c);
+    pair_of.assign((size_t)nq, 0);
+    for (int p = 0; p < n_pairs; p++)
+        for (int i = qo[p]; i < qo[p + 1]; i++) pair_of[i] = p;
+    int rc;
+    if ((rc = ensure(c, S.q, (size_t)nq * 32)) || (rc = ensure(c, S.t, (size_t)nt * 32)) || (rc = ensure(c, S.pairq, (size_t)nq * 4)) ||
+        (rc = ensure(c, S.toff, (size_t)(n_pairs + 1) * 4)))
+        return rc;
+    if (cudaMemcpyAsync(S.q.p, query32, (size_t)nq * 32, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(S.t.p, train32, (size_t)nt * 32, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(S.pairq.p, pair_of.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(S.toff.p, to, (size_t)(n_pairs + 1) * 4, cudaMemcpyHostToDevice, st) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "upload of the descriptors failed");
+    return CS_OK;
+}
+
+/* a sorted-match launch: room for out_off[nq] keys at S.mkeys, offsets uploaded to S.moff, counts at S.mcnt; with out_off == NULL the
+ * counting launch (no keys, no shared memory) */
+int launch_sorted(cs_ctx *c, LbdState &S, int nq, int max_dist, const std::vector<long long> *out_off, int max_m)
+{
+    cudaStream_t st = cs_ctx_stream(c);
+    int rc;
+    if ((rc = ensure(c, S.mcnt, (size_t)nq * 4))) return rc;
+    unsigned sort_cap = 0;
+    if (out_off) {
+        sort_cap = 1;
+        while ((int)sort_cap < max_m) sort_cap <<= 1;
+        if ((rc = ensure(c, S.mkeys, (size_t)(*out_off)[nq] * 8)) || (rc = ensure(c, S.moff, (size_t)(nq + 1) * 8))) return rc;
+        if (cudaMemcpyAsync(S.moff.p, out_off->data(), (size_t)(nq + 1) * 8, cudaMemcpyHostToDevice, st) != cudaSuccess)
+            return cs_ctx_fail(c, CS_ERR_CUDA, "upload of the match offsets failed");
+    }
+    launch_lbd_match_sorted((unsigned)nq, st, sort_cap, (const uint4 *)S.q.p, (const uint4 *)S.t.p, (const int32_t *)S.pairq.p, (const int32_t *)S.toff.p, nq,
+                            max_dist, out_off ? (const long long *)S.moff.p : nullptr, out_off ? (unsigned long long *)S.mkeys.p : nullptr, (int32_t *)S.mcnt.p);
+    cs_ctx_count_launches(c, 1);
+    if (cudaGetLastError() != cudaSuccess) return cs_ctx_fail(c, CS_ERR_CUDA, "matcher kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return CS_OK;
+}
+
+/* cv::DMatch of a key, as match() builds it; beyond D = 128 the reference never writes results[], and the library reports train_idx -1 */
+void key_to_dmatch(unsigned long long key, int query_idx, cs_dmatch &m)
+{
+    const int d = CS_LBD_KEY_DIST(key);
+    m.query_idx = query_idx;
+    m.train_idx = d <= 128 ? (int32_t)CS_LBD_KEY_TRAIN(key) : -1;
+    m.img_idx = 0;
+    m.distance = (float)d;
+}
+
 }  // namespace
 
 void cs_lbd_destroy(void *state)
 {
     LbdState *S = (LbdState *)state;
-    Buf *all[] = {&S->lines, &S->desc, &S->fdesc, &S->coef, &S->q, &S->t, &S->pairq, &S->toff, &S->keys};
+    Buf *all[] = {&S->lines, &S->desc, &S->fdesc, &S->coef, &S->q, &S->t, &S->pairq, &S->toff, &S->keys, &S->mkeys, &S->moff, &S->mcnt};
     for (Buf *b : all)
         if (b->p) cudaFree(b->p);
     delete S;
@@ -378,6 +450,132 @@ int cs_match_line_descrip(cs_ctx *c, const uint8_t *query32, int n_query, const 
     if (n_query < 0 || n_train < 0 || !n_matches) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "bad descriptor counts");
     const int32_t qo[2] = {0, n_query}, to[2] = {0, n_train};
     return cs_match_line_descrip_batch(c, query32, qo, train32, to, 1, thres, matches, n_matches);
+}
+
+int cs_knn_match_line_descrip_batch(cs_ctx *c, const uint8_t *query32, const int32_t *query_offsets, const uint8_t *train32, const int32_t *train_offsets,
+                                    int n_pairs, int k, const uint8_t *query_mask, cs_dmatch *matches, int32_t *n_per_query)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    int rc = check_pairs(c, query_offsets, train_offsets, n_pairs);
+    if (rc) return rc;
+    if (k < 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "k must not be negative");
+    const int nq = query_offsets[n_pairs], nt = train_offsets[n_pairs];
+    if (nq > 0 && !n_per_query) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null n_per_query");
+    for (int i = 0; i < nq; i++) n_per_query[i] = 0;
+    if (nq == 0 || nt == 0 || k == 0) return CS_OK; /* "descriptors matrices cannot be void" (:270-274); k = 0: no entry per query */
+    if (!query32 || !train32 || !matches) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null descriptors or output");
+    cudaSetDevice(cs_ctx_device(c));
+    cudaStream_t st = cs_ctx_stream(c);
+    LbdState &S = *state_of(c);
+    std::vector<int32_t> pair_of;
+    if ((rc = upload_pairs(c, S, query32, query_offsets, train32, train_offsets, n_pairs, pair_of))) return rc;
+    auto keep = [&](int i) { return !query_mask || query_mask[i]; };
+    if (k <= 2) {
+        if ((rc = ensure(c, S.mkeys, (size_t)nq * 16))) return rc;
+        launch_lbd_knn2((unsigned)nq, st, (const uint4 *)S.q.p, (const uint4 *)S.t.p, (const int32_t *)S.pairq.p, (const int32_t *)S.toff.p, nq,
+                        (unsigned long long *)S.mkeys.p);
+        cs_ctx_count_launches(c, 1);
+        if (cudaGetLastError() != cudaSuccess) return cs_ctx_fail(c, CS_ERR_CUDA, "matcher kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+        std::vector<unsigned long long> keys((size_t)nq * 2);
+        if (cudaMemcpyAsync(keys.data(), S.mkeys.p, keys.size() * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+            return cs_ctx_fail(c, CS_ERR_CUDA, "match copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+        for (int i = 0; i < nq; i++) {
+            if (!keep(i)) continue;
+            int n = 0;
+            while (n < k && keys[2 * (size_t)i + n] != ~0ull) {
+                key_to_dmatch(keys[2 * (size_t)i + n], i - query_offsets[pair_of[i]], matches[(size_t)i * k + n]);
+                n++;
+            }
+            n_per_query[i] = n;
+        }
+        return CS_OK;
+    }
+    /* k > 2: min(k, train set) slots per kept query, the first of its sorted met codes */
+    std::vector<long long> off((size_t)nq + 1, 0);
+    int max_nt = 0;
+    for (int i = 0; i < nq; i++) {
+        const int ntp = train_offsets[pair_of[i] + 1] - train_offsets[pair_of[i]];
+        const int room = keep(i) ? std::min(k, ntp) : 0;
+        off[i + 1] = off[i] + room;
+        if (room) max_nt = std::max(max_nt, ntp);
+    }
+    if (off[nq] == 0) return CS_OK;
+    if ((rc = launch_sorted(c, S, nq, 256 /* every met code */, &off, max_nt))) return rc;
+    std::vector<unsigned long long> keys((size_t)off[nq]);
+    std::vector<int32_t> cnt((size_t)nq);
+    if (cudaMemcpyAsync(keys.data(), S.mkeys.p, keys.size() * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaMemcpyAsync(cnt.data(), S.mcnt.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "match copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+    for (int i = 0; i < nq; i++) {
+        for (int j = 0; j < cnt[i]; j++) key_to_dmatch(keys[(size_t)off[i] + j], i - query_offsets[pair_of[i]], matches[(size_t)i * k + j]);
+        n_per_query[i] = cnt[i];
+    }
+    return CS_OK;
+}
+
+int cs_knn_match_line_descrip(cs_ctx *c, const uint8_t *query32, int n_query, const uint8_t *train32, int n_train, int k, const uint8_t *query_mask,
+                              cs_dmatch *matches, int32_t *n_per_query)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    if (n_query < 0 || n_train < 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "bad descriptor counts");
+    const int32_t qo[2] = {0, n_query}, to[2] = {0, n_train};
+    return cs_knn_match_line_descrip_batch(c, query32, qo, train32, to, 1, k, query_mask, matches, n_per_query);
+}
+
+int cs_radius_match_line_descrip_batch(cs_ctx *c, const uint8_t *query32, const int32_t *query_offsets, const uint8_t *train32, const int32_t *train_offsets,
+                                       int n_pairs, float max_distance, const uint8_t *query_mask, cs_dmatch *matches, int64_t max_matches,
+                                       int64_t *match_offsets)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    int rc = check_pairs(c, query_offsets, train_offsets, n_pairs);
+    if (rc) return rc;
+    if (!match_offsets || max_matches < 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null match_offsets or negative max_matches");
+    const int nq = query_offsets[n_pairs], nt = train_offsets[n_pairs];
+    for (int i = 0; i <= nq; i++) match_offsets[i] = 0;
+    /* k_distances[j] <= maxDistance (:484): an integer distance against a float; NaN and negative radii take nothing */
+    const int max_dist = !(max_distance >= 0.0f) ? -1 : (max_distance >= 256.0f ? 256 : (int)floorf(max_distance));
+    if (nq == 0 || nt == 0 || max_dist < 0) return CS_OK;
+    if (!query32 || !train32) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null descriptors");
+    cudaSetDevice(cs_ctx_device(c));
+    cudaStream_t st = cs_ctx_stream(c);
+    LbdState &S = *state_of(c);
+    std::vector<int32_t> pair_of;
+    if ((rc = upload_pairs(c, S, query32, query_offsets, train32, train_offsets, n_pairs, pair_of))) return rc;
+    /* first launch: how many codes each query has within the radius */
+    if ((rc = launch_sorted(c, S, nq, max_dist, nullptr, 0))) return rc;
+    std::vector<int32_t> cnt((size_t)nq);
+    if (cudaMemcpyAsync(cnt.data(), S.mcnt.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "match count copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+    std::vector<long long> off((size_t)nq + 1, 0);
+    int max_m = 0;
+    for (int i = 0; i < nq; i++) {
+        const int m = (!query_mask || query_mask[i]) ? cnt[i] : 0;
+        off[i + 1] = off[i] + m;
+        max_m = std::max(max_m, m);
+    }
+    for (int i = 0; i <= nq; i++) match_offsets[i] = off[i];
+    if (off[nq] > max_matches)
+        return cs_ctx_fail(c, CS_ERR_CAPACITY, "%lld matches within the radius exceed max_matches = %lld; match_offsets holds the layout they need",
+                           (long long)off[nq], (long long)max_matches);
+    if (off[nq] == 0) return CS_OK;
+    if (!matches) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null matches");
+    /* second launch: the codes themselves, sorted, at their offsets */
+    if ((rc = launch_sorted(c, S, nq, max_dist, &off, max_m))) return rc;
+    std::vector<unsigned long long> keys((size_t)off[nq]);
+    if (cudaMemcpyAsync(keys.data(), S.mkeys.p, keys.size() * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "match copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+    for (int i = 0; i < nq; i++)
+        for (long long j = off[i]; j < off[i + 1]; j++) key_to_dmatch(keys[(size_t)j], i - query_offsets[pair_of[i]], matches[j]);
+    return CS_OK;
+}
+
+int cs_radius_match_line_descrip(cs_ctx *c, const uint8_t *query32, int n_query, const uint8_t *train32, int n_train, float max_distance,
+                                 const uint8_t *query_mask, cs_dmatch *matches, int64_t max_matches, int64_t *match_offsets)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    if (n_query < 0 || n_train < 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "bad descriptor counts");
+    const int32_t qo[2] = {0, n_query}, to[2] = {0, n_train};
+    return cs_radius_match_line_descrip_batch(c, query32, qo, train32, to, 1, max_distance, query_mask, matches, max_matches, match_offsets);
 }
 
 }  // extern "C"

@@ -3,13 +3,124 @@
 detect_filter_lines(img) -> n x 4 float32 [x1 y1 x2 y2]: what the reference writes into its `cv::Mat& linesmat_out`
 (line_lbd/class/line_lbd_allclass.cpp:216-221).  The descriptor / matcher methods (get_line_descriptors, detect_descrip_lines,
 detect_descrip_lines_octaves, match_line_descrip; :191-198,224-356) return numpy arrays: key lines as records of `_lib.KEYLINE_DTYPE`
-(the KeyLine fields, octave 0), descriptors as n x 32 uint8 (the CV_8UC1 matrix), matches as records of `_lib.DMATCH_DTYPE` (cv::DMatch)."""
+(the KeyLine fields, octave 0), descriptors as n x 32 uint8 (the CV_8UC1 matrix), matches as records of `_lib.DMATCH_DTYPE` (cv::DMatch).
+`line_lbd_detect.bdm` is the class's BinaryDescriptorMatcher (line_lbd_allclass.h:37): pairwise match, knnMatch and radiusMatch on the GPU."""
 import ctypes as C
+import math
 
 import numpy as np
 
 from . import _lib
 from .detect_3d_cuboid import Context, CubeSlamError
+
+
+def _codes(d):
+    return np.ascontiguousarray(d, np.uint8).reshape(-1, 32)
+
+
+class BinaryDescriptorMatcher(object):
+    """Mirror of cv::line_descriptor::BinaryDescriptorMatcher, the pairwise forms (binary_descriptor_matcher.cpp:196-341, 431-507), on the
+    device of `context`.  Descriptors are n x 32 uint8; a list of matches is a records array of `_lib.DMATCH_DTYPE`, a vector<vector<DMatch>>
+    a Python list of them, one per query.  mask: one value per query (0 = skip it), its length must be the number of queries.  Where the
+    reference is undefined the library's definitions hold (include/cube_slam_b200.h): fewer than k entries when fewer codes are met,
+    train_idx -1 beyond 128 bits, [] for an empty query or train set.  At most 16384 train codes per pair (CubeSlamError beyond)."""
+
+    def __init__(self, context):
+        self._ctx = context
+
+    @staticmethod
+    def _mask(mask, n):
+        if mask is None:
+            return None
+        m = np.asarray(mask).reshape(-1)
+        if len(m) != n:
+            raise CubeSlamError("mask has %d entries for %d query descriptors" % (len(m), n))
+        return np.ascontiguousarray(m != 0, np.uint8)
+
+    def _pack(self, queries, trains, masks):
+        qs, ts = [_codes(q) for q in queries], [_codes(t) for t in trains]
+        if len(qs) != len(ts) or not qs:
+            raise CubeSlamError("one train set per query set, at least one pair")
+        masks = [None] * len(qs) if masks is None else list(masks)
+        if len(masks) != len(qs):
+            raise CubeSlamError("one mask (or None) per pair")
+        ms = [self._mask(m, len(q)) for m, q in zip(masks, qs)]
+        qo = np.concatenate([[0], np.cumsum([len(q) for q in qs])]).astype(np.int32)
+        to = np.concatenate([[0], np.cumsum([len(t) for t in ts])]).astype(np.int32)
+        q = np.ascontiguousarray(np.concatenate(qs)) if qo[-1] else np.zeros((1, 32), np.uint8)
+        t = np.ascontiguousarray(np.concatenate(ts)) if to[-1] else np.zeros((1, 32), np.uint8)
+        m = None
+        if any(x is not None for x in ms):
+            m = np.ascontiguousarray(np.concatenate([x if x is not None else np.ones(len(qq), np.uint8) for x, qq in zip(ms, qs)] + [np.zeros(1, np.uint8)]))
+        return qs, ts, ms, q, qo, t, to, m
+
+    def match(self, queryDescriptors, trainDescriptors, mask=None):
+        """match(query, train, matches, mask): the nearest code of every (unmasked) query -> DMATCH_DTYPE records, query order."""
+        q, t = _codes(queryDescriptors), _codes(trainDescriptors)
+        m = self._mask(mask, len(q))
+        out = np.zeros(max(len(q), 1), _lib.DMATCH_DTYPE)
+        n = C.c_int32(0)
+        self._ctx.check(self._ctx.L.cs_match_line_descrip(self._ctx.h, _lib.ptr(q, C.c_uint8), len(q), _lib.ptr(t, C.c_uint8), len(t), C.c_float(math.inf),
+                                                          out.ctypes.data, C.byref(n)))
+        out = out[:n.value].copy()
+        return out if m is None else out[m[out["query_idx"]] != 0]
+
+    def knnMatch(self, queryDescriptors, trainDescriptors, k, mask=None, compactResult=False):
+        """knnMatch(query, train, matches, k, mask, compactResult): per query its first k codes; a masked query gives an empty list, or
+        none with compactResult."""
+        return self.knnMatch_batch([queryDescriptors], [trainDescriptors], k, None if mask is None else [mask], compactResult)[0]
+
+    def radiusMatch(self, queryDescriptors, trainDescriptors, maxDistance, mask=None, compactResult=False):
+        """radiusMatch(query, train, matches, maxDistance, mask, compactResult): per query every code at distance <= maxDistance; with
+        compactResult empty lists are left out."""
+        return self.radiusMatch_batch([queryDescriptors], [trainDescriptors], maxDistance, None if mask is None else [mask], compactResult)[0]
+
+    def knnMatch_batch(self, queries, trains, k, masks=None, compactResult=False):
+        """knnMatch over independent (query set, train set) pairs in one launch -> one vector<vector<DMatch>> per pair."""
+        qs, ts, ms, q, qo, t, to, m = self._pack(queries, trains, masks)
+        k = int(k)
+        kk = min(k, max(len(x) for x in ts)) if k > 0 else k     # no query gets more entries than its train set has codes
+        nq = int(qo[-1])
+        out = np.zeros(max(nq * kk, 1), _lib.DMATCH_DTYPE)
+        n = np.zeros(max(nq, 1), np.int32)
+        self._ctx.check(self._ctx.L.cs_knn_match_line_descrip_batch(self._ctx.h, _lib.ptr(q, C.c_uint8), _lib.ptr(qo, C.c_int32), _lib.ptr(t, C.c_uint8),
+                                                                    _lib.ptr(to, C.c_int32), len(qs), kk, None if m is None else _lib.ptr(m, C.c_uint8),
+                                                                    out.ctypes.data, _lib.ptr(n, C.c_int32)))
+        res = []
+        for p in range(len(qs)):
+            if not len(qs[p]) or not len(ts[p]):
+                res.append([])
+                continue
+            res.append([out[i * kk:i * kk + n[i]].copy() for i in range(qo[p], qo[p + 1])
+                        if not (compactResult and ms[p] is not None and not ms[p][i - qo[p]])])
+        return res
+
+    def radiusMatch_batch(self, queries, trains, maxDistance, masks=None, compactResult=False, max_matches=None):
+        """radiusMatch over independent pairs in one call -> one vector<vector<DMatch>> per pair.  max_matches: the first buffer's size
+        (default 8 per query); when the matches do not fit, the call is repeated once with the size the library reports."""
+        qs, ts, ms, q, qo, t, to, m = self._pack(queries, trains, masks)
+        nq = int(qo[-1])
+        cap = int(max_matches) if max_matches is not None else 8 * nq
+        off = np.zeros(nq + 1, np.int64)
+        L, h = self._ctx.L, self._ctx.h
+        for attempt in range(2):
+            out = np.zeros(max(cap, 1), _lib.DMATCH_DTYPE)
+            rc = L.cs_radius_match_line_descrip_batch(h, _lib.ptr(q, C.c_uint8), _lib.ptr(qo, C.c_int32), _lib.ptr(t, C.c_uint8), _lib.ptr(to, C.c_int32),
+                                                      len(qs), C.c_float(maxDistance), None if m is None else _lib.ptr(m, C.c_uint8), out.ctypes.data,
+                                                      C.c_int64(cap), _lib.ptr(off, C.c_int64))
+            if rc == -3 and attempt == 0 and off[-1] > cap:        # CS_ERR_CAPACITY with the layout filled: resize and call again
+                cap = int(off[-1])
+                continue
+            self._ctx.check(rc)
+            break
+        res = []
+        for p in range(len(qs)):
+            if not len(qs[p]) or not len(ts[p]):
+                res.append([])
+                continue
+            lists = [out[off[i]:off[i + 1]].copy() for i in range(qo[p], qo[p + 1])]
+            res.append([x for x in lists if len(x) or not compactResult])
+        return res
 
 
 class line_lbd_detect(object):
@@ -19,6 +130,11 @@ class line_lbd_detect(object):
         self.use_LSD = False            # line_lbd_allclass.cpp:121
         self.line_length_thres = 50.0   # :122
         self._ctx = context if context is not None else Context(device, max_width, max_height, 1, 1, 1)
+
+    @property
+    def bdm(self):
+        """The class's BinaryDescriptorMatcher (line_lbd_allclass.h:37, created at :117), on this detector's context."""
+        return BinaryDescriptorMatcher(self._ctx)
 
     def params(self):
         p = _lib.LineParams()

@@ -327,6 +327,35 @@ int cs_match_line_descrip(cs_ctx *ctx, const uint8_t *query32, int n_query, cons
 int cs_match_line_descrip_batch(cs_ctx *ctx, const uint8_t *query32, const int32_t *query_offsets, const uint8_t *train32,
                                 const int32_t *train_offsets, int n_pairs, float matching_dist_thres, cs_dmatch *matches, int32_t *n_matches);
 
+/* BinaryDescriptorMatcher::knnMatch(query, train, matches, k, mask, compactResult) and radiusMatch(query, train, matches, maxDistance, mask,
+ * compactResult) (line_lbd/libs/binary_descriptor_matcher.cpp:264-341, 431-507) -- the pairwise forms, as line_lbd_detect::bdm offers them.
+ * A query's answer comes in the order of the reference's multi-index hash (distance first, then the order the hash meets equally near codes,
+ * as in cs_match_line_descrip): knn the first k codes, radius every code at distance <= max_distance (note <=, where match_line_descrip
+ * keeps distance < thres).  query_idx / train_idx count within the pair, img_idx is 0.  What the reference leaves undefined is defined here:
+ *   - only codes the hash meets count (a code none of whose 32 bytes is within 4 bits of the query's is never met), so a query may get
+ *     fewer than k entries -- the reference returns k with uninitialised ones;
+ *   - a code in the answer further than 128 bits away reports train_idx -1 (the reference never writes its trainIdx), distance as it is;
+ *   - an empty query or train set gives no entries (the reference prints and returns); k = 0 gives none; k < 0 is CS_ERR_INVALID_ARG.
+ * query_mask (NULL: every query; else one byte per query, 0 = skip) follows the reference's mask: a skipped query gets no entries.  Whether
+ * such a query shows as an empty list (compactResult) is the caller's view of n_per_query / match_offsets.
+ * Every pair's train set holds at most CS_LBD_KNN_MAX_TRAIN = 16384 codes (the sorting kernel stages a query's keys in 128 KB of shared
+ * memory); a larger one is CS_ERR_CAPACITY.
+ * knn: matches has room for n_queries x k entries; query i's n_per_query[i] entries start at matches[i * k] (the rest of its row is left as
+ * it is).  k <= 2, what a ratio test asks for, takes a kernel of its own that keeps the two best in registers.
+ * radius: the entries of query i are matches[match_offsets[i] .. match_offsets[i + 1]), query after query, in matches[0 .. max_matches).
+ * When they do not fit the call returns CS_ERR_CAPACITY with match_offsets (n_queries + 1) filled, so match_offsets[n_queries] is the
+ * size to call again with. */
+int cs_knn_match_line_descrip(cs_ctx *ctx, const uint8_t *query32, int n_query, const uint8_t *train32, int n_train, int k, const uint8_t *query_mask,
+                              cs_dmatch *matches, int32_t *n_per_query);
+int cs_knn_match_line_descrip_batch(cs_ctx *ctx, const uint8_t *query32, const int32_t *query_offsets, const uint8_t *train32,
+                                    const int32_t *train_offsets, int n_pairs, int k, const uint8_t *query_mask, cs_dmatch *matches,
+                                    int32_t *n_per_query);
+int cs_radius_match_line_descrip(cs_ctx *ctx, const uint8_t *query32, int n_query, const uint8_t *train32, int n_train, float max_distance,
+                                 const uint8_t *query_mask, cs_dmatch *matches, int64_t max_matches, int64_t *match_offsets);
+int cs_radius_match_line_descrip_batch(cs_ctx *ctx, const uint8_t *query32, const int32_t *query_offsets, const uint8_t *train32,
+                                       const int32_t *train_offsets, int n_pairs, float max_distance, const uint8_t *query_mask,
+                                       cs_dmatch *matches, int64_t max_matches, int64_t *match_offsets);
+
 /* tests: what the host side hands the descriptor kernel -- per key line {mid x, mid y, cos, sin, length, frame} (6 x 4 bytes) -- and the
  * two Gaussian weight tables F_g (63) and F_l (21) as floats (binary_descriptor.cpp:140-179).  Host-only, needs no context. */
 int cs_lbd_debug_prepare(const cs_keyline *keylines, int n, void *lines24, float *coef_g63, float *coef_l21);
