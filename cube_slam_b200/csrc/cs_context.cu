@@ -66,11 +66,9 @@ struct cs_ctx {
     std::vector<int32_t> dt_ids, tile_job;
     int dt_class_off[CS_DT_CLASSES + 1] = {0}, dt_class_plane_words[CS_DT_CLASSES] = {0};
     int64_t total_px = 0, total_cand = 0, total_bits = 0;
-    int n_tiles = 0, max_plane_words = 0, max_dpitch = 0, max_roi_h = 0;
+    int n_tiles = 0, max_plane_words = 0, max_dpitch = 0;
     int use_raster_dt = 0; /* A/B: two-pass raster-scan distance transform instead of the cone form */
     bool use_tma = true;       /* tile kernels of the line detectors: interior tiles staged by the copy engine (cp.async.bulk.tensor); bit 8 of cs_set_profiling turns it off */
-    bool use_tma_canny = false; /* the same in k_canny_nms: no faster than the byte loads on H100 (c3 stage 0.287 vs 0.288 ms; the kernel is bound by integer ALU work, not by its loads), so opt-in: bit 9 */
-    int use_fused_dt = 0; /* experimental: fused hysteresis + wavefront DT kernel */
     cudaStream_t stream2 = nullptr; /* side stream: the line kernel runs beside the image chain */
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     /* the skinny, latency-bound tail of the chain (distance transform -> sweep -> selection: a few warps per SM, long dependent chains) runs on
@@ -210,7 +208,6 @@ int build_tables(cs_ctx *c)
     c->n_tiles = 0;
     c->max_plane_words = 0;
     c->max_dpitch = 0;
-    c->max_roi_h = 0;
     const int img_width = c->w, img_height = c->h;
 
     for (int f = 0; f < F; f++) {
@@ -333,7 +330,6 @@ int build_tables(cs_ctx *c)
                 c->total_bits += 2 * (int64_t)plane_words;
                 c->max_plane_words = std::max(c->max_plane_words, plane_words);
                 c->max_dpitch = std::max(c->max_dpitch, jb.dpitch);
-                c->max_roi_h = std::max(c->max_roi_h, jb.roi_h);
                 jb.cand_off = c->total_cand;
                 c->total_cand += jb.n_cand;
                 jb.tile_off = c->n_tiles;
@@ -468,14 +464,10 @@ int run_batch(cs_ctx *c, bool sync)
         gray = (const uint8_t *)c->d_img.p;
     mark(ST_CANNY);
     int low = (int)std::floor(std::min(c->prm.canny_low, c->prm.canny_high)), high = (int)std::floor(std::max(c->prm.canny_low, c->prm.canny_high));
-    cs_launch_canny(gray, c->w, c->h, c->n_frames, (const CsJob *)c->d_jobs.p, n_jobs, (const int32_t *)c->d_tilejob.p, (int)c->tile_job.size(), (uint32_t *)c->d_bits.p,
-                    (size_t)c->total_bits * 4, low, high, (int32_t *)c->d_err.p, c->use_tma_canny, st, &c->launches);
+    cs_launch_canny(gray, c->w, c->h, (const CsJob *)c->d_jobs.p, n_jobs, (const int32_t *)c->d_tilejob.p, (int)c->tile_job.size(), (uint32_t *)c->d_bits.p,
+                    (size_t)c->total_bits * 4, low, high, st, &c->launches);
     mark(ST_HYST);
-    bool fused = false;
-    if (c->use_fused_dt)
-        fused = cs_launch_hyst_dt((const CsJob *)c->d_jobs.p, n_jobs, (uint32_t *)c->d_bits.p, (float *)c->d_dist.p, c->max_plane_words, c->max_dpitch,
-                                  c->max_roi_h, st, &c->launches);
-    if (!fused) cs_launch_hyst((const CsJob *)c->d_jobs.p, n_jobs, (uint32_t *)c->d_bits.p, c->max_plane_words, st, &c->launches);
+    cs_launch_hyst((const CsJob *)c->d_jobs.p, n_jobs, (uint32_t *)c->d_bits.p, c->max_plane_words, st, &c->launches);
     mark(ST_DT);
     const bool tail_hi = c->use_prio && !c->profiling;
     if (tail_hi) { /* hand the rest of the chain to the high-priority stream */
@@ -483,9 +475,8 @@ int run_batch(cs_ctx *c, bool sync)
         st = c->stream_hi;
         cudaStreamWaitEvent(st, c->ev_mid, 0);
     }
-    if (!fused)
-        cs_launch_dt((const CsJob *)c->d_jobs.p, (const int32_t *)c->d_dtids.p, n_jobs, c->max_dpitch, c->dt_class_off, c->dt_class_plane_words, (const uint32_t *)c->d_bits.p,
-                     (float *)c->d_dist.p, c->use_raster_dt, st, c->stream2, c->ev_dt_fork, c->ev_dt_join, &c->launches);
+    cs_launch_dt((const CsJob *)c->d_jobs.p, (const int32_t *)c->d_dtids.p, n_jobs, c->max_dpitch, c->dt_class_off, c->dt_class_plane_words, (const uint32_t *)c->d_bits.p,
+                 (float *)c->d_dist.p, c->use_raster_dt, st, c->stream2, c->ev_dt_fork, c->ev_dt_join, &c->launches);
     mark(ST_LINES);
     cudaStreamWaitEvent(st, c->ev_join, 0); /* join */
     mark(ST_SWEEP);
@@ -1058,12 +1049,10 @@ int cs_set_profiling(cs_ctx *c, int enable)
 {
     if (!c) return CS_ERR_INVALID_ARG;
     c->profiling = (enable & 1) != 0;
-    c->use_fused_dt = (enable & 4) != 0; /* bit 2: experimental fused hysteresis + wavefront-DT kernel */
     c->use_raster_dt = ((enable & 32) ? 1 : 0) | ((enable & 64) ? 2 : 0); /* bit 5: raster-scan distance transform kernel; bit 6: cone form, bits from global */
     c->use_prio = (enable & 16) == 0;      /* bit 4: keep the whole chain on one stream (no high-priority tail) */
     c->seq_lines = (enable & 128) != 0;    /* bit 7: sequential seed loop / routing of the line detectors (A/B reference of the speculative kernels) */
     c->use_tma = (enable & 256) == 0;      /* bit 8: the line detectors' tile kernels stage every tile with byte loads (A/B of the TMA path) */
-    c->use_tma_canny = (enable & 512) != 0; /* bit 9: k_canny_nms stages interior gray tiles by TMA as well */
     c->use_cta_select = (enable & 8) != 0; /* bit 3: CTA-wide sweep / selection kernels (the general path) instead of the warp ones */
     c->carry_cam_pose = (enable & 1024) != 0; /* bit 10: cs_detect_cuboids[_batch] carries the reference's cam_pose from box to box of a sampled frame */
     return CS_OK;

@@ -1476,18 +1476,8 @@ int ed_ensure(cs_ctx *c, Buf &b, size_t bytes)
 inline int ed_grid(int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, CS_SM_COUNT * 32); }
 /* nodes of a frame's walk graph that k_ed_route keeps in shared memory (4 bytes + 1 bit each): 32,766 = the 15-bit id limit, one frame
  * per SM (H100, c3 EDLines with 12 batches in flight: 3.66 ms per step, 4.14 with 26,000 -- two frames per SM, where the densest frames
- * of a batch fall back to walking in HBM);
- * CS_ED_SM_NODES overrides for A/B runs */
-inline int ed_sm_nodes()
-{
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("CS_ED_SM_NODES");
-        v = e ? atoi(e) : 32766;
-        v = std::max(1024, std::min(v, 32766));
-    }
-    return v;
-}
+ * of a batch fall back to walking in HBM) */
+#define ED_SM_NODES 32766
 
 EdState *ed_state_of(cs_ctx *c)
 {
@@ -1579,7 +1569,7 @@ static int ed_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_fra
     }
     /* the walk graph, routing on it, chains fitted in parallel, segments in order (see the comment above k_ed_rowcount) */
     const int dev = cs_ctx_device(c);
-    int sm_nodes = ed_sm_nodes();
+    const int sm_nodes = ED_SM_NODES;
     const size_t sm_bytes = (size_t)sm_nodes * 4 + (size_t)((sm_nodes + 31) / 32) * 4 + (size_t)ED_SM_ANCHORS * 2;
     if (dev >= 0 && dev < 64 && !S.route_attr_set[dev]) {
         cudaFuncSetAttribute(k_ed_route, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_bytes);

@@ -8,9 +8,9 @@
 #include "cs_internal.h"
 
 /* One shared-memory carveout for every kernel of the chain: kernels of several batches share the SMs, and an SM only changes its
- * L1 / shared split when it is idle.  Default 75 (% shared); -1 leaves the driver's per-kernel choice (CS_SMEM_CARVEOUT in the environment overrides;
- * it is a preference: a kernel that needs more shared memory still gets it). */
-int cs_carveout_pref(void);
+ * L1 / shared split when it is idle.  75 % shared (a preference: a kernel that needs more shared memory still gets it).  H100, c3
+ * headline with 12 batches in flight: 8.75 ms per step at 75 % shared, 9.06 with the driver's per-kernel choice. */
+#define CS_SMEM_CARVEOUT_PCT 75
 /* Function attributes are per device: `cs_first_on_device(flags)` is true the first time it runs on the current device (the flag word is
  * a bit per device ordinal, updated atomically: contexts on several devices / host threads may launch the same kernel). */
 #include <atomic>
@@ -39,9 +39,8 @@ static inline void cs_allow_max_dynamic_smem(K kernel)
         return;
     cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)a.sharedSizeBytes);
 }
-#define CS_APPLY_CARVEOUT(kernel)                                                                                                     \
-    CS_ONCE_PER_DEVICE(const int cv_ = cs_carveout_pref();                                                                            \
-                       if (cv_ >= 0) cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cv_))
+#define CS_APPLY_CARVEOUT(kernel) \
+    CS_ONCE_PER_DEVICE(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, CS_SMEM_CARVEOUT_PCT))
 
 #define CS_DT_CLASSES 7
 extern const int cs_dt_class_width[CS_DT_CLASSES];
@@ -49,14 +48,12 @@ int cs_dt_class_of(int roi_w);
 
 void cs_launch_gray(const uint8_t *d_img, uint8_t *d_gray, int n_frames, int w, int h, int stride, int channels, cudaStream_t st,
                     int64_t *launches);
-void cs_launch_canny(const uint8_t *d_gray, int img_w, int img_h, int n_frames, const CsJob *d_jobs, int n_jobs, const int32_t *d_tile_job, int n_tiles,
-                     uint32_t *d_bits, size_t bits_bytes, int low, int high, int32_t *d_err, bool use_tma, cudaStream_t st, int64_t *launches);
+void cs_launch_canny(const uint8_t *d_gray, int img_w, int img_h, const CsJob *d_jobs, int n_jobs, const int32_t *d_tile_job, int n_tiles,
+                     uint32_t *d_bits, size_t bits_bytes, int low, int high, cudaStream_t st, int64_t *launches);
 void cs_launch_hyst(const CsJob *d_jobs, int n_jobs, uint32_t *d_bits, int max_plane_words, cudaStream_t st, int64_t *launches);
 void cs_launch_dt(const CsJob *d_jobs, const int32_t *d_ids, int n_jobs, int max_dpitch, const int *class_off, const int *class_plane_words,
                   const uint32_t *d_bits, float *d_dist, int raster_or_flags, cudaStream_t st, cudaStream_t st_side, cudaEvent_t ev_fork,
                   cudaEvent_t ev_join, int64_t *launches);
-bool cs_launch_hyst_dt(const CsJob *d_jobs, int n_jobs, uint32_t *d_bits, float *d_dist, int max_plane_words, int max_dpitch, int max_h,
-                       cudaStream_t st, int64_t *launches);
 void cs_launch_roi_lines(const CsJob *d_jobs, int n_jobs, const CsFrame *d_frames, const double *d_lines, const float *d_lines_f32,
                          const int32_t *d_n_lines_dev, int f32_pitch, double *d_out_lines,
                          int32_t *d_out_counts, int32_t *d_err, double dist_thre, double angle_thre_deg, double len_thre, cudaStream_t st,

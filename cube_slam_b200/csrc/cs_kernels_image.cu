@@ -13,10 +13,7 @@
  * zero border: (h+2) rows of (bw+2) 32-bit words, bw = ceil(w/32).  That makes NMS output two ballots per
  * warp, hysteresis a word-parallel dilation in shared memory, and the distance transform's input 32x smaller.
  */
-#include <cuda.h>
 #include <cuda_runtime.h>
-#include <string.h>
-#include <stdlib.h>
 #include <stdint.h>
 
 #include "cs_internal.h"
@@ -73,25 +70,14 @@ __global__ void __launch_bounds__(256) k_bgr2gray_generic(const uint8_t *__restr
  * in shared memory; magnitudes of the +1 halo are held there too (zero outside the ROI).  A warp
  * owns 32 consecutive pixels of a row, so the strong / weak classification leaves as two ballots.
  * ------------------------------------------------------------------------------------------ */
-#define CT 32 /* tile edge */
+#define CT 32  /* tile edge */
+#define CTP 64 /* pitch of the staged gray tile in bytes (36 used) */
 
-/* TMA staging of the gray tile (kTma): a tile whose 36 x 36 halo region lies inside the ROI needs no clamping, so one elected thread
- * asks the copy engine for it (cp.async.bulk.tensor.2d, box 64 x 36 bytes of the {width, frames x height} gray tensor, completion on
- * an mbarrier) one tile ahead, into the other half of a double buffer.  The innermost start coordinate of a box must be a multiple of
- * 16 bytes (anything else is an illegal-instruction fault, cs_tma.cuh), so the box starts at the tile's x rounded
- * down and the tile is read at an offset of 0..15 bytes; tiles that touch the ROI border (cv::Canny on gray(roi) replicates
- * the ROI's own border, TMA would zero-fill or read the neighbours) keep the clamped byte loads.  The tile pitch is 48 bytes either way. */
-#define CTP 64 /* pitch of the staged gray tile in bytes: 36 used + up to 15 of alignment slack (a TMA box starts at a multiple of 16 bytes) */
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-template <bool kTma>
-__global__ void __launch_bounds__(256) k_canny_nms(const __grid_constant__ CUtensorMap tmap, const uint8_t *__restrict__ gray, int img_w, int img_h,
-                                                   const CsJob *__restrict__ jobs, const int32_t *__restrict__ tile_job, uint32_t *__restrict__ bits_arena,
-                                                   int low, int high, int32_t *__restrict__ err_flag)
+__global__ void __launch_bounds__(256) k_canny_nms(const uint8_t *__restrict__ gray, int img_w, int img_h, const CsJob *__restrict__ jobs,
+                                                   const int32_t *__restrict__ tile_job, uint32_t *__restrict__ bits_arena, int low, int high)
 {
-    /* gray, +2 halo, two buffers; a TMA destination must be 128-byte aligned: 36 rows x 48 bytes = 1728, padded to 1792 */
+    /* gray, +2 halo: 36 rows at a pitch of CTP bytes, in two buffers that alternate from tile to tile */
     __shared__ __align__(128) uint8_t s_gb_raw[2][((CT + 4) * CTP + 127) / 128 * 128];
-    __shared__ __align__(8) unsigned long long s_bar[2];
     __shared__ int32_t s_d[CT + 2][CT + 2 + 1];   /* (dy << 16) | (dx & 0xffff), +1 halo */
     __shared__ uint16_t s_m[CT + 2][CT + 2 + 2];  /* |dx| + |dy|, zero outside the ROI */
     /* a block owns one ROW of tiles of one ROI and walks it left to right; the gray bytes of the next tile are fetched into
@@ -112,9 +98,7 @@ __global__ void __launch_bounds__(256) k_canny_nms(const __grid_constant__ CUten
     const uint16_t *mflat = &s_m[0][0];
     constexpr int NPRE = ((CT + 4) * (CT + 4) + 255) / 256;
     uint8_t pre[NPRE];
-    const bool rows_inside = (y0 - 2 >= 0) && (y0 + CT + 1 <= h - 1);
-    auto interior = [&](int x0) { return kTma && rows_inside && (x0 - 2 >= 0) && (x0 + CT + 1 <= w - 1); };
-    auto fetch = [&](int x0) { /* clamped byte loads into registers (ROI border tiles, or no TMA) */
+    auto fetch = [&](int x0) { /* clamped byte loads into registers */
 #pragma unroll
         for (int q = 0; q < NPRE; q++) {
             const int i = tid + q * 256;
@@ -127,63 +111,21 @@ __global__ void __launch_bounds__(256) k_canny_nms(const __grid_constant__ CUten
             }
         }
     };
-    auto tma_issue = [&](int x0, int buf) { /* one thread: arm the barrier with the byte count, start the copy */
-        const uint32_t bar = smem_u32(&s_bar[buf]), dst = smem_u32(&s_gb_raw[buf][0]);
-        const int cx = (jb.roi_l + x0 - 2) & ~15, cy = jb.frame * img_h + jb.roi_t + y0 - 2; /* start rounded down to 16 bytes */
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); /* the buffer was last read through the generic proxy */
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)((CT + 4) * CTP)) : "memory");
-        asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
-                     "l"(reinterpret_cast<uint64_t>(&tmap)), "r"(cx), "r"(cy), "r"(bar)
-                     : "memory");
-    };
-    uint32_t phase0 = 0, phase1 = 0; /* parity of the next completion of either barrier */
-    if (kTma) {
-        if (tid == 0) {
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&s_bar[0])) : "memory");
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&s_bar[1])) : "memory");
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncthreads();
-    }
-    bool cur_tma = interior(0);
-    if (cur_tma) {
-        if (tid == 0) tma_issue(0, 0);
-    } else
-        fetch(0);
+    fetch(0);
     for (int tile_x = 0; tile_x < tiles_x; tile_x++) {
         const int x0 = tile_x * CT;
         const int buf = tile_x & 1;
         uint8_t(*s_g)[CTP] = reinterpret_cast<uint8_t(*)[CTP]>(&s_gb_raw[buf][0]);
-        const int goff = cur_tma ? ((jb.roi_l + x0 - 2) & 15) : 0; /* where the tile starts inside the staged rows */
-        if (cur_tma) { /* wait for the copy engine: every thread polls the barrier's phase (bounded: a lost copy must not hang the GPU) */
-            const uint32_t bar = smem_u32(&s_bar[buf]);
-            const uint32_t parity = buf ? phase1 : phase0;
-            uint32_t done = 0;
-            for (int spin = 0; spin < (1 << 22) && !done; spin++)
-                asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}" : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-            if (!done && tid == 0) atomicOr(err_flag, 8);
-            if (buf)
-                phase1 ^= 1u;
-            else
-                phase0 ^= 1u;
-        } else {
 #pragma unroll
-            for (int q = 0; q < NPRE; q++) {
-                const int i = tid + q * 256;
-                if (i < (CT + 4) * (CT + 4)) {
-                    const int ly = i / (CT + 4), lx = i - ly * (CT + 4);
-                    s_g[ly][lx] = pre[q];
-                }
+        for (int q = 0; q < NPRE; q++) {
+            const int i = tid + q * 256;
+            if (i < (CT + 4) * (CT + 4)) {
+                const int ly = i / (CT + 4), lx = i - ly * (CT + 4);
+                s_g[ly][lx] = pre[q];
             }
         }
         __syncthreads();
-        if (tile_x + 1 < tiles_x) { /* the next tile, into the other buffer (everybody left it before the barrier above) */
-            cur_tma = interior(x0 + CT);
-            if (cur_tma) {
-                if (tid == 0) tma_issue(x0 + CT, buf ^ 1);
-            } else
-                fetch(x0 + CT);
-        }
+        if (tile_x + 1 < tiles_x) fetch(x0 + CT); /* the next tile, into registers */
         /* Sobel + magnitude for the (CT+2)^2 halo region: a thread owns one column and a strip of 5 rows, the three-row
          * window slides down in registers (21 shared loads for 5 results) */
         int loud = 0; /* does any pixel of the tile proper exceed the low threshold? (the +1 halo ring does not count) */
@@ -194,7 +136,7 @@ __global__ void __launch_bounds__(256) k_canny_nms(const __grid_constant__ CUten
 #pragma unroll
             for (int r = 0; r < 7; r++) {
                 const int row = min(r0 + r, CT + 3);
-                const int a = s_g[row][goff + lx], b = s_g[row][goff + lx + 1], c = s_g[row][goff + lx + 2];
+                const int a = s_g[row][lx], b = s_g[row][lx + 1], c = s_g[row][lx + 2];
                 rs[r] = a + 2 * b + c;
                 rd[r] = c - a;
             }
@@ -906,177 +848,6 @@ __global__ void __launch_bounds__(32 * (2 + 2 * DT_NC), (NCH <= 3 ? 3 : (NCH <= 
     }
 }
 
-/* ------------------------------------------------------------------------------------------
- * Fused hysteresis + chamfer distance transform, one CTA per ROI (the default path).
- *
- * Hysteresis as in k_canny_hyst, with both bit planes in shared memory.  The distance transform then
- * runs as a skewed WAVEFRONT instead of a row-by-row scan: warp b owns the 32-row band b, lane l owns
- * row 32b+l and walks it left to right, two columns behind the lane above it, so that the three
- * upper neighbours of every cell were produced one, two and three steps earlier:
- *       t(i,j) = min(t(i-1,j-1)+b, t(i-1,j)+a, t(i-1,j+1)+b, t(i,j-1)+a)        (0 on an edge pixel)
- * The value a lane just produced reaches the lane below with one __shfl_up; the last row of a band
- * reaches the next band's warp through a tagged word in shared memory (value | tag << 30), which the
- * consumer lane polls -- no block-wide barrier inside a pass.  Bands therefore pipeline: a ROI of
- * H x W finishes in about 2H + W steps while every SM keeps thousands of lanes busy.  Same integer
- * recurrences as the raster scan, evaluated in another order, hence bit-exact.
- * ------------------------------------------------------------------------------------------ */
-#define WF_BIG (1 << 29)
-#define WF_MAX_WARPS 16
-#define WF_SLACK 24
-
-template <bool BWD>
-__device__ __forceinline__ void wf_pass(const uint32_t *S /* smem edge plane, bordered */, int bwp, uint32_t *__restrict__ tmp, int w, int h,
-                                        int dpitch, volatile uint32_t *rowbuf /* nw x rb_pitch */, int rb_pitch, int nw)
-{
-    const unsigned FULL = 0xffffffffu;
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int nbands = (h + 31) >> 5;
-    const float scale = 1.f / 65536.f;
-    const float dist_max = (float)(0xffffffffu - (uint32_t)DT_DG) * scale;
-    for (int band = wid; band < nbands; band += nw) {
-        const int rr = band * 32 + lane; /* row in pass order */
-        const bool row_ok = rr < h;
-        const int r = BWD ? (h - 1 - rr) : rr;
-        const uint32_t tag_out = (uint32_t)(((band / nw) & 1) + 1) << 30;
-        const uint32_t tag_in = (band > 0) ? (uint32_t)((((band - 1) / nw) & 1) + 1) << 30 : 0u;
-        volatile uint32_t *rb_out = rowbuf + (size_t)(band % nw) * rb_pitch;
-        volatile uint32_t *rb_in = rowbuf + (size_t)((band + nw - 1) % nw) * rb_pitch;
-        const bool feeds_next = (band + 1 < nbands);
-        uint32_t *trow = tmp + (size_t)(row_ok ? r : 0) * dpitch;
-        const uint32_t *srow = S + (size_t)((row_ok ? r : 0) + 1) * bwp + 1;
-        int a = WF_BIG, b = WF_BIG, left = WF_BIG, last = WF_BIG;
-        uint32_t bits = 0;
-        uint32_t o0 = 0, o1 = 0, o2 = 0, o3 = 0;     /* forward: last four results of this row */
-        uint4 cg = make_uint4(WF_BIG, WF_BIG, WF_BIG, WF_BIG), ng = cg, ng2 = cg, ng3 = cg; /* backward: forward values, 3 groups ahead */
-        if (BWD && row_ok) {
-            const int g0 = (w - 1) & ~3;
-            cg = *reinterpret_cast<const uint4 *>(trow + g0);
-            if (g0 >= 4) ng = *reinterpret_cast<const uint4 *>(trow + g0 - 4);
-            if (g0 >= 8) ng2 = *reinterpret_cast<const uint4 *>(trow + g0 - 8);
-            if (g0 >= 12) ng3 = *reinterpret_cast<const uint4 *>(trow + g0 - 12);
-        }
-        /* start a band only once the band above is WF_SLACK columns ahead: afterwards both advance at the
-         * same rate and the per-step poll below finds its word ready (polling warps would otherwise eat
-         * the issue slots of the producers) */
-        if (band > 0 && lane == 0) {
-            const int need = min(WF_SLACK, w - 1);
-            while ((rb_in[need] & 0xc0000000u) != tag_in) __nanosleep(200);
-        }
-        __syncwarp();
-        int c_pref = WF_BIG; /* lane 0: upper-row value for the NEXT step, fetched one step early */
-        if (band > 0 && lane == 0) {
-            const uint32_t v = rb_in[0];
-            c_pref = (int)(v & 0x3fffffffu); /* column 0 is ready: need >= 0 */
-        }
-        const int n_steps = w + 64;
-        for (int s = 0; s < n_steps; s++) {
-            const int j = s - 2 * lane - 1; /* column in pass order; -1 = priming step */
-            int c = __shfl_up_sync(FULL, last, 1);
-            if (lane == 0) {
-                c = (band > 0) ? c_pref : WF_BIG;
-                if (band > 0 && j + 2 < w) { /* prefetch column j+2 for the next step */
-                    uint32_t v = rb_in[j + 2];
-                    while ((v & 0xc0000000u) != tag_in) {
-                        __nanosleep(100);
-                        v = rb_in[j + 2];
-                    }
-                    c_pref = (int)(v & 0x3fffffffu);
-                }
-            }
-            if (j + 1 >= w) c = WF_BIG;
-            if (row_ok && j >= 0 && j < w) {
-                const int col = BWD ? (w - 1 - j) : j;
-                int t = min(min(a + DT_DG, b + DT_HV), min(c + DT_DG, left + DT_HV));
-                if (!BWD) {
-                    if ((col & 31) == 0) bits = srow[col >> 5];
-                    if ((bits >> (col & 31)) & 1u) t = 0;
-                } else {
-                    const int q = col & 3;
-                    const uint32_t cur = (q == 3) ? cg.w : (q == 2) ? cg.z : (q == 1) ? cg.y : cg.x;
-                    t = min(t, (int)cur);
-                }
-                if (t >= WF_BIG) t = WF_BIG;
-                left = t;
-                last = t;
-                if (lane == 31 && feeds_next) rb_out[j] = (uint32_t)t | tag_out;
-                if (!BWD) {
-                    o0 = o1;
-                    o1 = o2;
-                    o2 = o3;
-                    o3 = (uint32_t)t;
-                    if ((col & 3) == 3)
-                        *reinterpret_cast<uint4 *>(trow + col - 3) = make_uint4(o0, o1, o2, o3);
-                    else if (col == w - 1) { /* ragged tail of the row */
-                        trow[col] = o3;
-                        if ((col & 3) >= 1) trow[col - 1] = o2;
-                        if ((col & 3) >= 2) trow[col - 2] = o1;
-                    }
-                } else {
-                    const float f = (t >= WF_BIG) ? dist_max : (float)(uint32_t)t * scale;
-                    const uint32_t fb = __float_as_uint(f);
-                    /* results leave in place of the forward values, a group of four at a time */
-                    const int q = col & 3;
-                    if (q == 3) o3 = fb;
-                    else if (q == 2) o2 = fb;
-                    else if (q == 1) o1 = fb;
-                    else o0 = fb;
-                    if (q == 0) {
-                        *reinterpret_cast<uint4 *>(trow + col) = make_uint4(o0, o1, o2, o3);
-                        cg = ng;
-                        ng = ng2;
-                        ng2 = ng3;
-                        if (col >= 16) ng3 = *reinterpret_cast<const uint4 *>(trow + col - 16);
-                    }
-                }
-            }
-            a = (j + 1 == 0) ? WF_BIG : b;
-            b = c;
-        }
-    }
-}
-
-extern __shared__ uint32_t hd_smem[];
-
-__global__ void __launch_bounds__(32 * WF_MAX_WARPS) k_hyst_dt(const CsJob *__restrict__ jobs, uint32_t *__restrict__ bits_arena,
-                                                               float *__restrict__ dist_arena, int plane_cap_words, int rb_pitch)
-{
-    const CsJob &jb = jobs[blockIdx.x];
-    const int h = jb.roi_h, w = jb.roi_w, bw = jb.bw, bwp = bw + 2;
-    const int plane = (h + 2) * bwp;
-    uint32_t *gS = bits_arena + jb.bit_off;
-    uint32_t *S = hd_smem;
-    uint32_t *W = S + plane;
-    uint32_t *rowbuf = hd_smem + 2 * plane_cap_words;
-    const int tid = threadIdx.x, nthreads = blockDim.x, nw = nthreads >> 5;
-    for (int i = tid; i < 2 * plane; i += nthreads) S[i] = gS[i];
-    for (int i = tid; i < nw * rb_pitch; i += nthreads) rowbuf[i] = 0;
-    __syncthreads();
-    /* hysteresis */
-    {
-        const int n_runs = max(nthreads / bw, 1);
-        const int rows_per = (h + n_runs - 1) / n_runs;
-        const int c = 1 + tid % bw, run = tid / bw;
-        const int r0 = 1 + run * rows_per, r1 = min(r0 + rows_per, h + 1);
-        const bool active = (run < n_runs) && (tid < n_runs * bw);
-        while (true) {
-            bool changed = false;
-            if (active) {
-                for (int r = r0; r < r1; r++) changed |= hyst_word<uint32_t *>(S, W, bwp, r, c);
-                for (int r = r1 - 2; r >= r0; r--) changed |= hyst_word<uint32_t *>(S, W, bwp, r, c);
-            }
-            if (!__syncthreads_or(changed ? 1 : 0)) break;
-        }
-        for (int i = tid; i < plane; i += nthreads) gS[i] = S[i]; /* final edge map (inspection / reuse) */
-    }
-    uint32_t *tmp = reinterpret_cast<uint32_t *>(dist_arena + jb.px_off);
-    wf_pass<false>(S, bwp, tmp, w, h, jb.dpitch, rowbuf, rb_pitch, nw);
-    __syncthreads(); /* forward values written by other warps' lanes are read back below */
-    for (int i = tid; i < nw * rb_pitch; i += nthreads) rowbuf[i] = 0;
-    __threadfence_block();
-    __syncthreads();
-    wf_pass<true>(S, bwp, tmp, w, h, jb.dpitch, rowbuf, rb_pitch, nw);
-}
-
 /* ------------------------------------------------------------------------------------------ launchers */
 /* ROI width classes of the distance transform: 1..5, 8 or 16 chunks of 128 columns (one kernel instantiation and one launch per class) */
 const int cs_dt_class_width[CS_DT_CLASSES] = {128, 256, 384, 512, 640, 1024, 2048};
@@ -1086,16 +857,6 @@ int cs_dt_class_of(int roi_w)
     for (int c = 0; c < CS_DT_CLASSES; c++)
         if (roi_w <= cs_dt_class_width[c]) return c;
     return -1;
-}
-
-int cs_carveout_pref(void)
-{
-    static int v = -2;
-    if (v == -2) {
-        const char *e = getenv("CS_SMEM_CARVEOUT");
-        v = e ? atoi(e) : 75; /* H100, c3 headline with 12 batches in flight: 8.75 ms per step at 75 % shared, 9.06 with the driver's choice */
-    }
-    return v;
 }
 
 void cs_launch_gray(const uint8_t *d_img, uint8_t *d_gray, int n_frames, int w, int h, int stride, int channels, cudaStream_t st,
@@ -1121,46 +882,14 @@ void cs_launch_gray(const uint8_t *d_img, uint8_t *d_gray, int n_frames, int w, 
     }
 }
 
-/* cuTensorMapEncodeTiled through the runtime (no link-time dependency on libcuda): the {width, frames x height} byte tensor of the gray
- * frames, box CTP x (CT + 4).  Returns false when the driver entry point is missing or the layout does not qualify (pitch not a multiple
- * of 16 bytes): the kernel then stages every tile with byte loads. */
-static bool cs_make_gray_tmap(CUtensorMap *tm, const uint8_t *d_gray, int img_w, int64_t rows)
-{
-    typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                                 const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    static EncodeFn fn = nullptr;
-    static bool tried = false;
-    if (!tried) {
-        tried = true;
-        void *p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess) fn = (EncodeFn)p;
-        cudaGetLastError();
-    }
-    if (!fn || (img_w % 16) != 0 || (((uintptr_t)d_gray) & 15) != 0 || img_w < CTP || rows < CT + 4) return false;
-    const cuuint64_t dims[2] = {(cuuint64_t)img_w, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)img_w};
-    const cuuint32_t box[2] = {CTP, CT + 4};
-    const cuuint32_t estr[2] = {1, 1};
-    return fn(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, (void *)d_gray, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-              CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-void cs_launch_canny(const uint8_t *d_gray, int img_w, int img_h, int n_frames, const CsJob *d_jobs, int n_jobs, const int32_t *d_tile_job, int n_tiles,
-                     uint32_t *d_bits, size_t bits_bytes, int low, int high, int32_t *d_err, bool use_tma, cudaStream_t st, int64_t *launches)
+void cs_launch_canny(const uint8_t *d_gray, int img_w, int img_h, const CsJob *d_jobs, int n_jobs, const int32_t *d_tile_job, int n_tiles,
+                     uint32_t *d_bits, size_t bits_bytes, int low, int high, cudaStream_t st, int64_t *launches)
 {
     if (n_jobs <= 0) return;
     cudaMemsetAsync(d_bits, 0, bits_bytes, st); /* zero borders (and stale bits) of every plane */
     if (n_tiles > 0) {
-        CUtensorMap tm;
-        memset(&tm, 0, sizeof(tm));
-        if (use_tma && cs_make_gray_tmap(&tm, d_gray, img_w, (int64_t)n_frames * img_h)) {
-            CS_APPLY_CARVEOUT(k_canny_nms<true>);
-            k_canny_nms<true><<<n_tiles, dim3(32, 8), 0, st>>>(tm, d_gray, img_w, img_h, d_jobs, d_tile_job, d_bits, low, high, d_err);
-        } else {
-            CS_APPLY_CARVEOUT(k_canny_nms<false>);
-            k_canny_nms<false><<<n_tiles, dim3(32, 8), 0, st>>>(tm, d_gray, img_w, img_h, d_jobs, d_tile_job, d_bits, low, high, d_err);
-        }
+        CS_APPLY_CARVEOUT(k_canny_nms);
+        k_canny_nms<<<n_tiles, dim3(32, 8), 0, st>>>(d_gray, img_w, img_h, d_jobs, d_tile_job, d_bits, low, high);
         (*launches)++;
     }
 }
@@ -1244,22 +973,4 @@ void cs_launch_dt(const CsJob *d_jobs, const int32_t *d_ids, int n_jobs, int max
         cudaEventRecord(ev_join, st_side);
         cudaStreamWaitEvent(st, ev_join, 0);
     }
-}
-
-/* fused hysteresis + wavefront DT; returns false if the batch's largest ROI does not fit shared memory
- * (the caller then uses cs_launch_hyst + cs_launch_dt) */
-bool cs_launch_hyst_dt(const CsJob *d_jobs, int n_jobs, uint32_t *d_bits, float *d_dist, int max_plane_words, int max_dpitch, int max_h,
-                       cudaStream_t st, int64_t *launches)
-{
-    if (n_jobs <= 0) return true;
-    int nw = (max_h + 31) / 32;
-    if (nw > WF_MAX_WARPS) nw = WF_MAX_WARPS;
-    if (nw < 2) nw = 2;
-    const int rb_pitch = (max_dpitch + 3) & ~3;
-    const size_t bytes = ((size_t)2 * max_plane_words + (size_t)nw * rb_pitch) * 4;
-    if (bytes > 200 * 1024) return false;
-    CS_ONCE_PER_DEVICE(cs_allow_max_dynamic_smem(k_hyst_dt));
-    k_hyst_dt<<<n_jobs, 32 * nw, bytes, st>>>(d_jobs, d_bits, d_dist, max_plane_words, rb_pitch);
-    (*launches)++;
-    return true;
 }

@@ -22,8 +22,8 @@
  *                    list, `used` as a bit per pixel in HBM read through L2).  Emits the candidate rectangles in seed order.
  *   k_lsd_val_count / k_lsd_val_nfa (six rounds)   rect_improve and the NFA test (lsd.cpp:520-534, 873-1136) read the angle map only: one
  *                    warp per undecided candidate rectangle, all frames at once; a round's up-to-five rectangles counted in one scan of the
- *                    angle map, the binomial tails in a kernel of their own (k_lsd_validate: the same as ONE kernel, kept as the A/B path --
- *                    its 6.6 k instructions do not fit the instruction cache, and its warps stall on instruction fetch).
+ *                    angle map, the binomial tails in a kernel of their own (as ONE kernel, its 6.6 k instructions would not fit the
+ *                    instruction cache, and its warps would stall on instruction fetch).
  *   k_lsd_emit       accepted candidates in seed order + the key-line filter.
  * Why this shape: the one-warp loop is bound by instruction issue, not by memory latency; what stops more frames from sharing an SM is the instruction cache, so the sequential kernel is
  * kept small (grow -> rectangle -> density is ONE two-pass loop, 7.4 k instructions instead of 39 k) and everything order-free runs where
@@ -61,7 +61,7 @@
 #define LSD_CHUNK_ROWS 8
 #define LSD_SCALE 0.8 /* lsd.cpp:459; k_lsd_front's tile spans assume it */
 
-#define LSD_CAND_CAP 2048    /* candidate rectangles per frame handed from the seed loop to k_lsd_validate, until a frame needs more */
+#define LSD_CAND_CAP 2048    /* candidate rectangles per frame handed from the seed loop to the validation kernels, until a frame needs more */
 #define LSD_SEQ_SCAP 2048    /* region entries k_lsd_grow_seq keeps in shared memory (the rest spill to HBM; small, so that many frames share an SM) */
 #define LSD_HDR 8            /* ints of a candidate record header in the arena: n1, n2, has_line, x1 y1 x2 y2 (float bits), pad */
 
@@ -304,7 +304,7 @@ struct LsdFrame {
     /* the `used` map as a bit per pixel (HBM, read and written through L2 only, so that it costs no shared memory: the seed loop issues
      * is bound by instruction issue, and the more frames share an SM the better) */
     uint32_t *ubits;
-    struct LsdSpan *span; /* k_lsd_validate: room for five row-span records per warp (shared memory) */
+    struct LsdSpan *span; /* k_lsd_val_count: room for five row-span records per warp (shared memory) */
     double *stage;        /* k_lsd_grow_seq: 96 doubles of shared memory per warp (ordered sums) */
     __device__ __forceinline__ bool used_bit(int addr) const { return (__ldcg(ubits + (addr >> 5)) >> (addr & 31)) & 1u; }
     const double *lgam; /* log_gamma of small integers (cs_nfa.cuh) */
@@ -868,86 +868,6 @@ __device__ void lsd_rect_count_multi(const LsdFrame &F, const LsdRect *r, int n,
     }
 }
 
-/* the NFA of up to five rectangles of one rect_improve phase: the pixel counts in one scan (rows across lanes), then the binomial tails,
- * each by the whole warp (cs_nfa.cuh) */
-__device__ __noinline__ void lsd_rect_nfa5(const LsdFrame &F, const LsdRect *r, int n, bool same_geom, double *v)
-{
-    int tot[5], alg[5];
-    {
-        LSD_PROF_T0();
-        if (n == 1)
-            lsd_rect_count(F, r[0], tot[0], alg[0]);
-        else
-            lsd_rect_count_multi(F, r, n, same_geom, tot, alg);
-        LSD_PROF_ADD(3);
-    }
-    {
-        LSD_PROF_T0();
-        for (int t = 0; t < n; t++) v[t] = cs_nfa_warp(F.lgam, tot[t], alg[t], r[t].p, F.LOG_NT, true); /* the whole warp on one binomial tail */
-        LSD_PROF_ADD(4);
-    }
-}
-
-/* lsd.cpp:873-975: the rectangles of a phase do not depend on the NFA values of that phase, so they are evaluated together */
-__device__ double lsd_rect_improve(const LsdFrame &F, LsdRect &rec)
-{
-    const double delta = 0.5, delta_2 = delta / 2.0, LOG_EPS = 0;
-    LsdRect cand[5];
-    double v[5];
-    lsd_rect_nfa5(F, &rec, 1, true, v);
-    double log_nfa = v[0];
-    if (log_nfa > LOG_EPS) return log_nfa;
-    LsdRect r = rec;
-    for (int n = 0; n < 5; ++n) {
-        r.p /= 2;
-        r.prec = r.p * LSD_PI;
-        cand[n] = r;
-    }
-    lsd_rect_nfa5(F, cand, 5, true, v);
-    for (int n = 0; n < 5; ++n)
-        if (v[n] > log_nfa) {
-            log_nfa = v[n];
-            rec = cand[n];
-        }
-    if (log_nfa > LOG_EPS) return log_nfa;
-    for (int phase = 0; phase < 4; phase++) {
-        r = rec;
-        int m = 0;
-        for (int n = 0; n < 5; ++n)
-            if ((r.width - delta) >= 0.5) {
-                if (phase == 0)
-                    r.width -= delta;
-                else if (phase == 1) {
-                    r.x1 += -r.dy * delta_2;
-                    r.y1 += r.dx * delta_2;
-                    r.x2 += -r.dy * delta_2;
-                    r.y2 += r.dx * delta_2;
-                    r.width -= delta;
-                } else if (phase == 2) {
-                    r.x1 -= -r.dy * delta_2;
-                    r.y1 -= r.dx * delta_2;
-                    r.x2 -= -r.dy * delta_2;
-                    r.y2 -= r.dx * delta_2;
-                    r.width -= delta;
-                } else {
-                    r.p /= 2;
-                    r.prec = r.p * LSD_PI;
-                }
-                cand[m++] = r;
-            }
-        if (m) {
-            lsd_rect_nfa5(F, cand, m, phase == 3, v);
-            for (int n = 0; n < m; ++n)
-                if (v[n] > log_nfa) {
-                    rec = cand[n];
-                    log_nfa = v[n];
-                }
-        }
-        if (phase < 3 && log_nfa > LOG_EPS) return log_nfa;
-    }
-    return log_nfa;
-}
-
 /* The first half of one seed (lsd.cpp:478-519): grow, rectangle, density refinement.  has_rect = 1 when a rectangle comes out that
  * rect_improve / the NFA test still have to judge -- which they can do later, in any order and in parallel: they read the level-line
  * angles only and never touch the `used` map. */
@@ -1037,27 +957,6 @@ __device__ void lsd_grow_candidate(const LsdFrame &F, const LsdReg &R, int s_add
     }
 }
 
-/* The second half (lsd.cpp:520-534): rect_improve, NFA test, back to image coordinates.  Returns whether the rectangle is a line. */
-__device__ bool lsd_validate_rect(const LsdFrame &F, LsdRect &rec, double scale, float *line)
-{
-    const double LOG_EPS = 0;
-    const double log_nfa = lsd_rect_improve(F, rec);
-    if (log_nfa <= LOG_EPS) return false;
-    rec.x1 += 0.5;
-    rec.y1 += 0.5;
-    rec.x2 += 0.5;
-    rec.y2 += 0.5;
-    rec.x1 /= scale;
-    rec.y1 /= scale;
-    rec.x2 /= scale;
-    rec.y2 /= scale;
-    line[0] = (float)rec.x1;
-    line[1] = (float)rec.y1;
-    line[2] = (float)rec.x2;
-    line[3] = (float)rec.y2;
-    return true;
-}
-
 /* checkLineExtremes + 10-px border rejection + length filter (LSDDetector.cpp:75-101,226-238; filter_lines): true = keep */
 __device__ __forceinline__ bool lsd_keyline_filter(const float *raw, int img_w, int img_h, float line_length_thres, float *o)
 {
@@ -1090,12 +989,8 @@ struct LsdGrowArgs {
     uint4 *pix;
     const float *angf;
     const double *modgrad;
-    const int32_t *list;
-    const int32_t *list_len;
-    uint32_t *st;
     int32_t *arena;
     int arena_cap;       /* ints per frame */
-    int32_t *spill;      /* LSD_SPILL ints per warp (the first LSD_SCAP unused) */
     double LOG_NT;
     int min_reg_size;
     double prec, p, scale;
@@ -1105,7 +1000,7 @@ struct LsdGrowArgs {
     float *out;
     int32_t *n_out;
     int cap;
-    LsdRect *cand;       /* cand_cap rectangles per frame, seed order: k_lsd_grow_seq -> k_lsd_validate */
+    LsdRect *cand;       /* cand_cap rectangles per frame, seed order: k_lsd_grow_seq -> k_lsd_val_count / k_lsd_val_nfa */
     int32_t *n_cand;
     int cand_cap;
     int32_t *cand_line;  /* per candidate: {is a line, 4 floats} */
@@ -1114,13 +1009,10 @@ struct LsdGrowArgs {
                           * [1]: the largest candidate count of a frame that overflowed, [2]: cand_cap */
     const double *lgam;  /* log_gamma table (cs_nfa.cuh) */
     uint32_t *ubits;     /* (W * H + 31) / 32 words per frame: the used map of k_lsd_grow_seq */
-    int32_t *redo;       /* per frame: 1 = the sequential kernel must redo this frame */
-    int32_t *stats;      /* per frame: rounds, candidates processed, refused, invalidated (diagnostics) */
 };
 
 /* The order-dependent half of the seed loop, one warp per frame (see the file header). */
-template <int kMinCtas>
-__global__ void __launch_bounds__(32, kMinCtas) k_lsd_grow_seq(LsdGrowArgs A, int scap)
+__global__ void __launch_bounds__(32, 21) k_lsd_grow_seq(LsdGrowArgs A, int scap)
 {
     const int f = blockIdx.x, lane = threadIdx.x;
     LSD_PROF_T0();
@@ -1178,7 +1070,7 @@ __global__ void __launch_bounds__(32, kMinCtas) k_lsd_grow_seq(LsdGrowArgs A, in
             LsdRect rec;
             lsd_grow_candidate(F, R, s_addr, A.min_reg_size, A.prec, A.p, n_all, has_rect, rec); /* arena_cap >= 2 W H: both passes fit */
             if (!has_rect) continue;
-            /* the rectangle goes to k_lsd_validate (rect_improve + NFA never touch the used map): candidates in seed order */
+            /* the rectangle goes to the validation kernels (rect_improve + NFA never touch the used map): candidates in seed order */
             if (lane == 0 && n_cand < A.cand_cap) A.cand[(size_t)f * A.cand_cap + n_cand] = rec;
             n_cand++;
         }
@@ -1195,43 +1087,9 @@ __global__ void __launch_bounds__(32, kMinCtas) k_lsd_grow_seq(LsdGrowArgs A, in
     LSD_PROF_ADD(6);
 }
 
-/* rect_improve + NFA of every candidate rectangle (lsd.cpp:520-534), one warp each: thousands of warps running the same code.  (A CTA of
- * five warps per candidate, one warp per rectangle of a rect_improve phase, was slower where it was timed; not re-timed on H100.) */
-template <int kMinCtas>
-__global__ void __launch_bounds__(128, kMinCtas) k_lsd_validate(LsdGrowArgs A)
-{
-    const int f = blockIdx.y, lane = threadIdx.x & 31;
-    const size_t npx = (size_t)A.W * A.H;
-    LsdFrame F;
-    F.W = A.W;
-    F.H = A.H;
-    F.pix = A.pix + f * npx;
-    F.angf = A.angf + f * npx;
-    F.modgrad = A.modgrad + f * npx;
-    F.LOG_NT = A.LOG_NT;
-    F.ubits = nullptr;
-    __shared__ LsdSpan s_span[4][5];
-    F.span = s_span[threadIdx.x >> 5];
-    F.stage = nullptr;
-    F.lgam = A.lgam;
-    F.wmagic = 0;
-    const int n = min(A.n_cand[f], A.cand_cap);
-    const int wpb = blockDim.x >> 5;
-    for (int c = blockIdx.x * wpb + (threadIdx.x >> 5); c < n; c += gridDim.x * wpb) {
-        LsdRect rec = A.cand[(size_t)f * A.cand_cap + c];
-        float line[4] = {0.f, 0.f, 0.f, 0.f};
-        const bool ok = lsd_validate_rect(F, rec, A.scale, line);
-        if (lane == 0) {
-            int32_t *o = A.cand_line + ((size_t)f * A.cand_cap + c) * 5;
-            o[0] = ok ? 1 : 0;
-            for (int k = 0; k < 4; k++) o[1 + k] = __float_as_int(line[k]);
-        }
-    }
-}
-
-/* ---- the same, split by phase into small kernels ---------------------------------------------------------------------------------
- * k_lsd_validate is ~6.6 k instructions (the scans, the double-precision log / exp / pow of the binomial tail, the improvement logic), the
- * L1.5 instruction cache holds 2 k, and its warps sit in different places of that code, so they stall on instruction fetch
+/* ---- rect_improve + NFA of every candidate rectangle (lsd.cpp:520-534), one warp each, split by phase into small kernels -----------
+ * As one kernel this would be ~6.6 k instructions (the scans, the double-precision log / exp / pow of the binomial tail, the improvement
+ * logic); the L1.5 instruction cache holds 2 k, and the warps would sit in different places of that code and stall on instruction fetch
  * (`no_instruction`).  rect_improve is six rounds of {count the pixels of up to five rectangles, turn the counts into NFA values, keep the
  * best} (lsd.cpp:873-975); run as twelve launches -- k_lsd_val_count(round), k_lsd_val_nfa(round) -- every warp of a launch is in the
  * same few hundred instructions.  State between launches: the candidate's current rectangle (A.cand, updated in place), its best
@@ -1370,12 +1228,7 @@ __global__ void __launch_bounds__(128, 5) k_lsd_val_nfa(LsdGrowArgs A, int round
     }
 }
 
-/* kernels one LSD run launches: front end, seed loop, validation (12 phase kernels, or the single kernel of the A/B variants), emit */
-static int cs_lsd_launches_per_run()
-{
-    static const int v_val = getenv("CS_LSD_VAL_VARIANT") ? atoi(getenv("CS_LSD_VAL_VARIANT")) : 0;
-    return 1 + 1 + (v_val == 0 ? 12 : 1) + 1;
-}
+#define LSD_LAUNCHES_PER_RUN 15 /* kernels one LSD run launches: front end, seed loop, 12 validation phase kernels, emit */
 
 /* the accepted candidates of a frame in seed order: raw segments, and those that pass the key-line filter */
 __global__ void __launch_bounds__(256) k_lsd_emit(LsdGrowArgs A)
@@ -1449,7 +1302,7 @@ struct Buf {
 
 struct LsdState {
     CsLineHead head; /* first: the error word (cs_internal.h) */
-    Buf img, modgrad, angf, pix, arena, raw, nraw, out, nout, redo, stats, lgam, ubits, cand, ncand, candline, candstate, err;
+    Buf img, modgrad, angf, pix, arena, raw, nraw, out, nout, lgam, ubits, cand, ncand, candline, candstate, err;
     bool lgam_filled = false;
     int last_frames = 0, last_W = 0, last_H = 0, cap = 0;
     /* the last run's frames (S.img, or the caller's device frames), from which cs_debug_lsd recomputes the scaled and modgrad planes */
@@ -1522,7 +1375,6 @@ int lsd_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, i
         (rc = ensure(c, S.arena, (size_t)n_frames * arena_cap * 4)) ||
         (rc = ensure(c, S.raw, (size_t)n_frames * cap * 16)) || (rc = ensure(c, S.nraw, (size_t)n_frames * 4)) ||
         (rc = ensure(c, S.out, (size_t)n_frames * cap * 16)) || (rc = ensure(c, S.nout, (size_t)n_frames * 4)) ||
-        (rc = ensure(c, S.redo, (size_t)n_frames * 4)) || (rc = ensure(c, S.stats, (size_t)n_frames * 16)) ||
         (rc = ensure(c, S.lgam, (size_t)CS_LGAMMA_TABLE * 8)) || (rc = ensure(c, S.ubits, (size_t)n_frames * (((size_t)W * H + 31) / 32) * 4)) ||
         (rc = ensure(c, S.cand, (size_t)n_frames * S.cand_cap * sizeof(LsdRect))) || (rc = ensure(c, S.ncand, (size_t)n_frames * 4)) ||
         (rc = ensure(c, S.candline, (size_t)n_frames * S.cand_cap * 20)) || (rc = ensure(c, S.candstate, (size_t)n_frames * S.cand_cap * sizeof(LsdCandState))) || (rc = ensure(c, S.err, 16)))
@@ -1543,7 +1395,6 @@ int lsd_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, i
     int32_t *const d_err = (int32_t *)S.err.p; /* the 16-byte error word (cs_internal.h) */
     S.head.d_err = d_err;
     cudaMemsetAsync(d_err, 0, 16, st);
-    cudaMemsetAsync(S.stats.p, 0, (size_t)n_frames * 16, st);
     lsd_front(c, d_img, n_frames, w, h, stride, channels, W, H, rho, (double *)S.modgrad.p, (float *)S.angf.p, (uint4 *)S.pix.p, nullptr, d_err);
     LsdGrowArgs A;
     A.W = W;
@@ -1553,12 +1404,8 @@ int lsd_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, i
     A.pix = (uint4 *)S.pix.p;
     A.angf = (const float *)S.angf.p;
     A.modgrad = (const double *)S.modgrad.p;
-    A.list = nullptr;
-    A.list_len = nullptr;
-    A.st = nullptr;
     A.arena = (int32_t *)S.arena.p;
     A.arena_cap = arena_cap;
-    A.spill = nullptr;
     A.LOG_NT = LOG_NT;
     A.min_reg_size = min_reg_size;
     A.prec = prec;
@@ -1578,32 +1425,15 @@ int lsd_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, i
     A.cand_line = (int32_t *)S.candline.p;
     A.cand_state = (LsdCandState *)S.candstate.p;
     A.err = d_err;
-    A.redo = (int32_t *)S.redo.p;
-    A.stats = (int32_t *)S.stats.p;
-    {
-        static const int v_grow = getenv("CS_LSD_GROW_VARIANT") ? atoi(getenv("CS_LSD_GROW_VARIANT")) : 0;
-        static const int v_val = getenv("CS_LSD_VAL_VARIANT") ? atoi(getenv("CS_LSD_VAL_VARIANT")) : 0;
-        static const int scap = getenv("CS_LSD_SCAP") ? atoi(getenv("CS_LSD_SCAP")) : LSD_SEQ_SCAP;
-        const size_t smem = (size_t)scap * 4 + 96 * 8; /* region list + the staging of the ordered sums (scap is even: 8-byte aligned) */
-        if (v_grow == 1)
-            k_lsd_grow_seq<32><<<n_frames, 32, smem, st>>>(A, scap);
-        else if (v_grow == 2)
-            k_lsd_grow_seq<25><<<n_frames, 32, smem, st>>>(A, scap);
-        else
-            k_lsd_grow_seq<21><<<n_frames, 32, smem, st>>>(A, scap);
-        /* 256 warps per frame: a warp per candidate for all but the densest frames */
-        if (v_val == 1)
-            k_lsd_validate<8><<<dim3(64, n_frames), 128, 0, st>>>(A);
-        else if (v_val == 2)
-            k_lsd_validate<5><<<dim3(64, n_frames), 128, 0, st>>>(A);
-        else
-            for (int round = 0; round < 6; round++) {
-                k_lsd_val_count<<<dim3(64, n_frames), 128, 0, st>>>(A, round);
-                k_lsd_val_nfa<<<dim3(64, n_frames), 128, 0, st>>>(A, round);
-            }
-        k_lsd_emit<<<n_frames, 256, 0, st>>>(A);
+    const size_t smem = (size_t)LSD_SEQ_SCAP * 4 + 96 * 8; /* region list + the staging of the ordered sums (LSD_SEQ_SCAP is even: 8-byte aligned) */
+    k_lsd_grow_seq<<<n_frames, 32, smem, st>>>(A, LSD_SEQ_SCAP);
+    /* 256 warps per frame: a warp per candidate for all but the densest frames */
+    for (int round = 0; round < 6; round++) {
+        k_lsd_val_count<<<dim3(64, n_frames), 128, 0, st>>>(A, round);
+        k_lsd_val_nfa<<<dim3(64, n_frames), 128, 0, st>>>(A, round);
     }
-    cs_ctx_count_launches(c, cs_lsd_launches_per_run());
+    k_lsd_emit<<<n_frames, 256, 0, st>>>(A);
+    cs_ctx_count_launches(c, LSD_LAUNCHES_PER_RUN);
     if (cudaGetLastError() != cudaSuccess) return cs_ctx_fail(c, CS_ERR_CUDA, "LSD kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
     S.last_frames = n_frames;
     S.last_W = W;
@@ -1673,7 +1503,7 @@ int cs_lsd_run_host(cs_ctx *c, const uint8_t *imgs, int n_frames, int w, int h, 
 void cs_lsd_destroy(void *state)
 {
     LsdState *S = (LsdState *)state;
-    Buf *all[] = {&S->img, &S->modgrad, &S->angf, &S->pix, &S->arena, &S->raw, &S->nraw, &S->out, &S->nout, &S->redo, &S->stats, &S->lgam, &S->ubits, &S->cand, &S->ncand, &S->candline, &S->candstate, &S->err};
+    Buf *all[] = {&S->img, &S->modgrad, &S->angf, &S->pix, &S->arena, &S->raw, &S->nraw, &S->out, &S->nout, &S->lgam, &S->ubits, &S->cand, &S->ncand, &S->candline, &S->candstate, &S->err};
     for (Buf *b : all)
         if (b->p) cudaFree(b->p);
     delete S;
@@ -1804,7 +1634,8 @@ int cs_debug_lsd(cs_ctx *c, int frame, int32_t *scaled_wh, double *scaled, doubl
 }
 
 /* cycle counters of the seed loop's phases summed over every warp since the last reset (diagnostics): {region_grow, region2rect, refine,
- * rectangle pixel counts, binomial tails, candidates grown, whole kernel (per CTA), unused} */
+ * rectangle pixel counts, binomial tails, candidates grown, whole kernel (per CTA), unused}.  Slots 3 and 4 read zero: the validation
+ * runs in the phase kernels, which keep no counters. */
 int cs_debug_lsd_prof(cs_ctx *c, uint64_t *out16, int reset)
 {
     if (!c) return CS_ERR_INVALID_ARG;
@@ -1818,18 +1649,16 @@ int cs_debug_lsd_prof(cs_ctx *c, uint64_t *out16, int reset)
     return cudaGetLastError() == cudaSuccess ? CS_OK : cs_ctx_fail(c, CS_ERR_CUDA, "debug copy failed");
 }
 
-/* diagnostics of the speculative seed loop of the last run: per frame {rounds, candidates processed, refused or lost, re-grown after an
- * override} and whether the sequential kernel redid the frame */
+/* kept for ABI stability (see the header): the seed loop runs one warp per frame with no speculative rounds, so stats4 reads zero and
+ * redo[f] = 1 */
 int cs_debug_lsd_stats(cs_ctx *c, int32_t *stats4, int32_t *redo, int n_frames)
 {
     if (!c) return CS_ERR_INVALID_ARG;
     LsdState *S = state_of(c);
     if (n_frames > S->last_frames) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "more frames than the last run held");
-    cudaSetDevice(cs_ctx_device(c));
-    cudaStreamSynchronize(cs_ctx_stream(c));
-    if (stats4) cudaMemcpy(stats4, S->stats.p, (size_t)n_frames * 16, cudaMemcpyDeviceToHost);
+    if (stats4) memset(stats4, 0, (size_t)n_frames * 16);
     if (redo)
-        for (int f = 0; f < n_frames; f++) redo[f] = 1; /* every frame goes through k_lsd_grow_seq (there is no speculative kernel any more) */
-    return cudaGetLastError() == cudaSuccess ? CS_OK : cs_ctx_fail(c, CS_ERR_CUDA, "debug copy failed");
+        for (int f = 0; f < n_frames; f++) redo[f] = 1;
+    return CS_OK;
 }
 }

@@ -209,7 +209,8 @@ class line_lbd_detect(object):
         return dict(scaled=sc, modgrad=mg, angles=an, list=lst[:ll.value].copy(), raw_lines=raw[:nr.value].copy())
 
     def seed_loop_stats(self, n_frames):
-        """Diagnostics of the last LSD run: (n_frames x 4 int32 {rounds, processed, refused, re-grown}, redo flags)."""
+        """Diagnostics of the last LSD run, kept for compatibility: (n_frames x 4 int32, all zero; redo flags, all 1 -- every frame
+        goes through the one-warp-per-frame seed loop)."""
         st, redo = np.zeros((n_frames, 4), np.int32), np.zeros(n_frames, np.int32)
         self._ctx.check(self._ctx.L.cs_debug_lsd_stats(self._ctx.h, _lib.ptr(st, C.c_int32), _lib.ptr(redo, C.c_int32), n_frames))
         return st, redo

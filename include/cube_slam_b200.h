@@ -219,12 +219,13 @@ void *cs_stream(cs_ctx *ctx);
 /* milliseconds spent in the named stage of the last cs_batch_run ("lsd","gray","canny","hyst","dt","lines","sweep","fuse","total") */
 int cs_stage_ms(cs_ctx *ctx, const char *stage, float *ms);
 /* bit 0: per-stage CUDA-event timing (adds event records only; the chain then stays on one stream).  Debug / A-B switches:
- * bit 2 fused hysteresis + wavefront distance transform, bit 3 CTA-wide sweep / selection kernels, bit 4 no high-priority
+ * bit 3 CTA-wide sweep / selection kernels, bit 4 no high-priority
  * stream for the distance transform -> sweep -> selection tail, bit 5 raster-scan distance transform (one kernel) instead of the cone form,
  * bit 6 cone-form distance transform reading the edge bits from global memory (the path of ROIs whose bit plane exceeds 96 KB),
  * bit 7 the line detectors' round-1 kernels (EDLines: routing and fitting on the pixel maps, one thread per frame) instead of the walk-graph
  * / warp-per-chain ones (the LSD seed loop has one form since the ordered-speculation kernel was measured and removed),
- * bit 8 byte-load staging in the line detectors' tile kernels (A/B of TMA), bit 9 TMA staging in the Canny kernel.
+ * bit 8 byte-load staging in the line detectors' tile kernels (A/B of TMA).  Bits 2 and 9 are accepted and ignored: they once selected
+ * kernel variants whose results were bit-identical to the default kernels', so callers that still pass them get the same output.
  * Mode switch, bit 10: with whether_sample_cam_roll_pitch the reference derives the yaw samples of box k + 1 of a frame from the
  * cam_pose box k left behind (box_proposal_detail.cpp:126-128 after :237,485) -- an ulp away from the raw pose's, which decides between 15
  * and 16 yaw samples.  By default every box starts from the raw pose (boxes independent, one pass); with bit 10
@@ -263,7 +264,8 @@ int cs_debug_lsd(cs_ctx *ctx, int frame, int32_t scaled_wh[2], double *scaled, d
 int cs_debug_lsd_stats(cs_ctx *ctx, int32_t *stats4, int32_t *redo, int n_frames);
 /* clock64 cycles the seed-loop warps spent per phase since the last reset (diagnostics; tools/time_lines.py): {region_grow, region2rect,
  * refine, rectangle pixel counts, binomial tails (nfa), seeds grown, whole kernel summed over CTAs, region pixels, and eight more slots of
- * finer counters inside region_grow} */
+ * finer counters inside region_grow}.  Slots 3 and 4 read zero: the rectangle counts and binomial tails run in the validation phase
+ * kernels, which keep no counters. */
 int cs_debug_lsd_prof(cs_ctx *ctx, uint64_t *out16, int reset);
 /* same for the EDLines flavour (use_LSD = 0): EDLineDetector's maps (binary_descriptor.cpp:1617-1666: blurred image, dxImg_, dyImg_,
  * gImgWO_ / 4, dirImg_), the anchors in scan order as y * width + x, the edge map after smart routing, the segments before the length filter */

@@ -27,7 +27,6 @@ void cs_edl_destroy(void *) {}
 void cs_lbd_destroy(void *) {}
 int cs_lsd_run_device(cs_ctx *c, const uint8_t *, int, int, int, int, int, float, int, const float **, const int32_t **) { return cs_ctx_fail(c, CS_ERR_UNSUPPORTED, "no line detector in this emulation"); }
 int cs_edl_run(cs_ctx *c, const uint8_t *, bool, int, int, int, int, int, float, int, const float **, const int32_t **) { return cs_ctx_fail(c, CS_ERR_UNSUPPORTED, "no line detector in this emulation"); }
-int cs_carveout_pref(void) { return -1; }
 const int cs_dt_class_width[CS_DT_CLASSES] = {128, 256, 384, 512, 640, 1024, 2048};
 int cs_dt_class_of(int roi_w)
 {
@@ -117,13 +116,12 @@ static void fill_from_oracle(cs_ctx *c)
 
 /* the launchers: every stage is a no-op except the last one of the chain */
 void cs_launch_gray(const uint8_t *, uint8_t *, int, int, int, int, int, cudaStream_t, int64_t *) {}
-void cs_launch_canny(const uint8_t *, int, int, int, const CsJob *, int, const int32_t *, int, uint32_t *, size_t, int, int, int32_t *, bool, cudaStream_t, int64_t *) {}
+void cs_launch_canny(const uint8_t *, int, int, const CsJob *, int, const int32_t *, int, uint32_t *, size_t, int, int, cudaStream_t, int64_t *) {}
 void cs_launch_hyst(const CsJob *, int, uint32_t *, int, cudaStream_t, int64_t *) {}
 void cs_launch_dt(const CsJob *, const int32_t *, int, int, const int *, const int *, const uint32_t *, float *, int, cudaStream_t, cudaStream_t, cudaEvent_t, cudaEvent_t,
                   int64_t *)
 {
 }
-bool cs_launch_hyst_dt(const CsJob *, int, uint32_t *, float *, int, int, int, cudaStream_t, int64_t *) { return true; }
 void cs_launch_roi_lines(const CsJob *, int, const CsFrame *, const double *, const float *, const int32_t *, int, double *, int32_t *, int32_t *, double, double, double,
                          cudaStream_t, int64_t *)
 {

@@ -126,7 +126,7 @@ def _border_batches(oracle, kw):
 
 @pytest.mark.parametrize("mode,kw", (("default", dict(max_cuboid_num=2)), ("height", dict(whether_sample_bbox_height=1, max_cuboid_num=2))))
 def test_border_and_small_boxes(cs, oracle, mode, kw):
-    """Default kernels, the raster-scan DT (bit 5), the cone DT with global bit planes (bit 6) and TMA-staged Canny tiles (bit 9)."""
+    """Default kernels, the raster-scan DT (bit 5) and the cone DT with global bit planes (bit 6)."""
     batches = _border_batches(oracle, kw)
     clamp = dict(left=0, right=0, top=0, bottom=0)
     n_no_cand = n_dup = n_neg = 0
@@ -146,7 +146,7 @@ def test_border_and_small_boxes(cs, oracle, mode, kw):
                 hs = E.height_samples(jb["box"], h)
                 n_dup += hs == [0, 0]
                 n_neg += min(hs) < 0
-        for flags in (0, 32, 64, 512):
+        for flags in (0, 32, 64):
             ctx = cs.Context(0, w, h, len(bt.frames), 10, 4096)
             bt.run(cs, ctx, flags)
             ctx.close()

@@ -88,11 +88,11 @@ def test_fixture_a_modes(cs, oracle, fixture_a, mode):
     ctx.close()
 
 
-@pytest.mark.parametrize("split_kernels", [0, 4, 32])
+@pytest.mark.parametrize("split_kernels", [0, 32])
 def test_fixture_a_stages(cs, oracle, fixture_a, split_kernels):
     """Stage by stage: gray/Canny/DT bit-exact, merged lines bit-exact, valid set + per-proposal errors.
-    Default: hysteresis kernel + cone-form distance transform (two sweeps + row scans).  4 selects the experimental fused
-    hysteresis + wavefront-DT kernel, 32 the two-pass raster-scan distance transform kernel."""
+    Default: hysteresis kernel + cone-form distance transform (two sweeps + row scans).  32 selects the two-pass raster-scan
+    distance transform kernel."""
     fa = fixture_a
     ctx = cs.Context(0, 1280, 960, 1, 8, 4096)
     ctx.L.cs_set_profiling(ctx.h, split_kernels)
@@ -120,8 +120,6 @@ def test_synthetic_batch_matches_oracle(cs, oracle, seed, w, h, kind, nb):
     imgs, Ts, boxes, lines, K = S.make_batch(seed, F, w, h, nb, kind=kind, poisson=(kind == "indoor"))
     ctx = cs.Context(0, w, h, F, 16, 4096)
     ctx.set_calibration(K)
-    if seed == 12:
-        ctx.L.cs_set_profiling(ctx.h, 4)  # one case through the fused wavefront kernel
     if seed == 11:
         ctx.L.cs_set_profiling(ctx.h, 8)  # one case through the CTA-wide sweep / selection kernels
     if seed == 13:
@@ -153,29 +151,22 @@ def test_synthetic_batch_matches_oracle(cs, oracle, seed, w, h, kind, nb):
     ctx.close()
 
 
-def test_canny_tma_staging_equals_byte_staging(cs, oracle):
-    """k_canny_nms<true> (cs_set_profiling bit 9: interior gray tiles fetched by the copy engine, cp.async.bulk.tensor + mbarrier; 640 and
-    1280 wide frames qualify) against k_canny_nms<false> (the default: every tile by clamped byte loads) and the oracle: same edge
-    bits, same records."""
+def test_canny_bits_match_oracle_on_every_roi(cs, oracle):
+    """k_canny_nms on every ROI of two multi-frame batches (640 x 480 and 1280 x 960, several ROIs per frame, interior and border
+    tiles): the edge bits equal the oracle's."""
     from cube_slam_b200 import synthetic as S
     for seed, w, h, nb in ((61, 640, 480, 4), (62, 1280, 960, 3)):
         imgs, Ts, boxes, lines, K = S.make_batch(seed, 3, w, h, nb, poisson=True)
-        outs = []
-        for flags in (0, 512):
-            ctx = cs.Context(0, w, h, 3, 16, 4096)
-            ctx.set_calibration(K)
-            ctx.L.cs_set_profiling(ctx.h, flags)
-            out, counts = ctx.detect_batch_host(imgs, Ts, boxes, lines, cs.default_params(max_cuboid_num=2))
-            rois = [ctx.debug_roi(j) for j in range(sum(len(b) for b in boxes))]
-            outs.append((out.copy(), counts.copy(), rois))
-            ctx.close()
-        assert outs[0][0].tobytes() == outs[1][0].tobytes() and (outs[0][1] == outs[1][1]).all()
+        ctx = cs.Context(0, w, h, 3, 16, 4096)
+        ctx.set_calibration(K)
+        ctx.detect_batch_host(imgs, Ts, boxes, lines, cs.default_params(max_cuboid_num=2))
+        rois = [ctx.debug_roi(j) for j in range(sum(len(b) for b in boxes))]
+        ctx.close()
         job = 0
         for f in range(3):
             for b in range(len(boxes[f])):
                 tr = oracle.detect_cuboid(imgs[f], K, Ts[f], boxes[f], lines[f], trace_object=b)["trace"]
-                for k in (0, 1):
-                    np.testing.assert_array_equal(outs[k][2][job]["canny"], tr["canny"])
+                np.testing.assert_array_equal(rois[job]["canny"], tr["canny"])
                 job += 1
 
 

@@ -113,7 +113,7 @@ def test_online_mode_with_edlines(det, oracle):
 
 # ---- shapes, strides and the three routing regimes ----------------------------------------------------------------------------------
 
-SM_NODES = 32766   # walk-graph nodes k_ed_route keeps in shared memory (cs_edlines.cu ed_sm_nodes)
+SM_NODES = 32766   # walk-graph nodes k_ed_route keeps in shared memory (cs_edlines.cu ED_SM_NODES)
 
 
 def routing_regime(oracle, img):

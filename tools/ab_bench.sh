@@ -1,5 +1,6 @@
 #!/bin/bash
-# A/B of environment-selected kernel variants inside ONE GPU-box session (boxes differ by a few per cent, so only same-box numbers compare).
+# A/B of environment settings (the variables bench.py only sets by default, such as CUDA_DEVICE_MAX_CONNECTIONS, and AB_INFLIGHT)
+# inside ONE GPU-box session (boxes differ by a few per cent, so only same-box numbers compare).
 # usage: tools/ab_bench.sh "<ENV=.. ENV=..>" "<...>" ...   prints ms/step of the headline path and the e2e figure per variant
 for v in "$@"; do
   AB_INFLIGHT=$(echo "$v" | sed -n 's/.*AB_INFLIGHT=\([0-9]*\).*/\1/p'); AB_INFLIGHT=${AB_INFLIGHT:-16}

@@ -1,5 +1,6 @@
 #!/bin/bash
-# N = 2 variants in one 2-GPU box session: tools/ab_bench_n2.sh "<ENV=..>" ...
+# N = 2 A/B of environment settings (the variables bench.py only sets by default, such as NCCL_MAX_NCHANNELS, and AB_INFLIGHT) in one 2-GPU box session:
+# tools/ab_bench_n2.sh "<ENV=..>" ...
 port=29520
 for v in "$@"; do
   port=$((port+1))

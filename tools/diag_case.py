@@ -1,6 +1,6 @@
 """Diagnostic: one synthetic test case through the cuboid path with a given cs_set_profiling flag, stage by stage against the oracle.
 
-    python tools/diag_case.py --seed 12 --flags 0 4
+    python tools/diag_case.py --seed 12 --flags 0 32
 """
 import argparse
 import os
@@ -15,7 +15,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--seed", type=int, default=12)
     ap.add_argument("--nb", type=int, default=5)
-    ap.add_argument("--flags", type=int, nargs="+", default=[0, 4])
+    ap.add_argument("--flags", type=int, nargs="+", default=[0, 32])
     ap.add_argument("--w", type=int, default=640)
     ap.add_argument("--h", type=int, default=480)
     ap.add_argument("--dump", default="")

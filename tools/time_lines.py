@@ -49,9 +49,6 @@ def main():
         sm = ctx.stage_ms()
         msg = "%s %s frames %d: line stage %.3f ms (CUDA events), whole step %.3f ms" % (args.flavour, "seq" if args.seq else "par", args.frames, sm["lsd"], sm["total"])
         if args.flavour == "lsd":
-            st, redo = det.seed_loop_stats(args.frames)
-            msg += " | (stats: %.0f %d %.0f %.0f %.0f %d)" % (
-                st[:, 0].mean(), st[:, 0].max(), st[:, 1].mean(), st[:, 2].mean(), st[:, 3].mean(), redo.sum())
             ctx.L.cs_debug_lsd_prof(ctx.h, prof.ctypes.data_as(C.POINTER(C.c_uint64)), 0)
             pf = prof.astype(np.float64) / args.frames
             msg += " | Mcycles/frame: grow %.2f rect %.2f refine %.2f count %.2f nfa %.2f kernel %.2f, seeds grown/frame %.0f, region px/frame %.0f" % (
