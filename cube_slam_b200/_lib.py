@@ -136,6 +136,10 @@ EXPORTS += DEVICE_FRAME_EXPORTS
 # k-nearest-neighbour and radius matching of line descriptors (cs_lbd.cu), bound the same way
 MATCHER_EXPORTS = ["cs_knn_match_line_descrip", "cs_knn_match_line_descrip_batch", "cs_radius_match_line_descrip", "cs_radius_match_line_descrip_batch"]
 EXPORTS += MATCHER_EXPORTS
+# matching against a device-resident collection of many images' codes (cs_lbd_collection.cu), bound the same way
+COLLECTION_EXPORTS = ["cs_lbd_collection_create", "cs_lbd_collection_destroy", "cs_lbd_collection_add", "cs_lbd_collection_clear",
+                      "cs_lbd_collection_size", "cs_lbd_collection_match", "cs_lbd_collection_knn_match", "cs_lbd_collection_radius_match"]
+EXPORTS += COLLECTION_EXPORTS
 
 
 def load():
@@ -207,6 +211,17 @@ def load():
         L.cs_knn_match_line_descrip_batch.argtypes = [vp, u8_p, i32_p, u8_p, i32_p, i, i, u8_p, vp, i32_p]
         L.cs_radius_match_line_descrip.argtypes = [vp, u8_p, i, u8_p, i, C.c_float, u8_p, vp, C.c_int64, i64_p]
         L.cs_radius_match_line_descrip_batch.argtypes = [vp, u8_p, i32_p, u8_p, i32_p, i, C.c_float, u8_p, vp, C.c_int64, i64_p]
+    if all(hasattr(L, n) for n in COLLECTION_EXPORTS):
+        L.cs_lbd_collection_create.restype = vp
+        L.cs_lbd_collection_create.argtypes = [vp]
+        L.cs_lbd_collection_destroy.restype = None
+        L.cs_lbd_collection_destroy.argtypes = [vp]
+        L.cs_lbd_collection_add.argtypes = [vp, u8_p, i32_p, i]
+        L.cs_lbd_collection_clear.argtypes = [vp]
+        L.cs_lbd_collection_size.argtypes = [vp, i32_p, i64_p]
+        L.cs_lbd_collection_match.argtypes = [vp, u8_p, i, u8_p, i, vp, i32_p]
+        L.cs_lbd_collection_knn_match.argtypes = [vp, u8_p, i, i, u8_p, i, vp, i32_p]
+        L.cs_lbd_collection_radius_match.argtypes = [vp, u8_p, i, C.c_float, u8_p, i, vp, C.c_int64, i64_p]
     L.cs_lbd_debug_prepare.argtypes = [vp, i, vp, f_p, f_p]
     L.cs_lbd_debug_keylines_edl.argtypes = [f_p, f_p, i, i, i, vp]
     L.cs_debug_last_set_pose.argtypes = [u8_p, d_p, d_p, i, i, i32_p]
@@ -217,7 +232,7 @@ def load():
         L.cs_batch_upload_online_device.argtypes = [vp, df_p, d_p, d_p, i32_p, C.POINTER(LineParams), C.POINTER(CuboidParams)]
         L.cs_detect_lines_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), f_p, C.c_int32, i32_p]
     for name in EXPORTS:
-        if name in DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS and not hasattr(L, name):
+        if name in DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS and not hasattr(L, name):
             continue
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("cs_abi_version",):

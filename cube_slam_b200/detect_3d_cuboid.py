@@ -6,6 +6,8 @@ read like calls into the reference.  All numerical work is done by the CUDA libr
 """
 import ctypes as C
 
+import weakref
+
 import numpy as np
 
 from . import _lib
@@ -53,6 +55,7 @@ class Context(object):
     """Owns one cs_ctx (one CUDA stream + device workspace).  One per host thread."""
 
     def __init__(self, device=0, max_width=1280, max_height=960, max_frames=1, max_boxes_per_frame=16, max_lines_per_frame=4096):
+        self._dependents = weakref.WeakSet()   # objects holding library state made on this context (descriptor collections)
         self.L = _lib.load()
         self.h = self.L.cs_create(device, max_width, max_height, max_frames, max_boxes_per_frame, max_lines_per_frame)
         if not self.h:
@@ -61,8 +64,14 @@ class Context(object):
 
     def close(self):
         if getattr(self, "h", None):
+            for obj in list(getattr(self, "_dependents", ())):   # the C ABI wants them released before the context
+                obj._release()
             self.L.cs_destroy(self.h)
             self.h = None
+
+    def _depend(self, obj):
+        """obj._release() frees what obj made on this context; close() calls it first"""
+        self._dependents.add(obj)
 
     def __del__(self):
         try:

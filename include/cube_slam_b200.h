@@ -358,6 +358,48 @@ int cs_radius_match_line_descrip_batch(cs_ctx *ctx, const uint8_t *query32, cons
                                        const int32_t *train_offsets, int n_pairs, float max_distance, const uint8_t *query_mask,
                                        cs_dmatch *matches, int64_t max_matches, int64_t *match_offsets);
 
+/* The collection forms of BinaryDescriptorMatcher ("from one image to a set", line_lbd/libs/binary_descriptor_matcher.cpp:70-104 add / train /
+ * clear, :126-193 match, :344-428 knnMatch, :510-595 radiusMatch): one query set against the codes of many images -- a keyframe map for
+ * relocalisation or loop closure -- that stay on the device between queries.
+ * A collection is created on a context and uses its device and stream; several collections may share one context.  Destroy every
+ * collection before its context (cs_lbd_collection_destroy reads the context).  clear() forgets every image and returns the collection's
+ * device memory (its codes and scratch buffers); the collection stays usable.  It holds fewer than 2^31 codes in all (CS_ERR_CAPACITY beyond), otherwise only device memory bounds it;
+ * there is no per-image or per-call cap on its size.
+ * add: n_images images whose codes are codes32[image_offsets[i] .. image_offsets[i + 1]) (32-byte rows, image_offsets has n_images + 1
+ * entries starting at 0), appended after what is there; uploaded on the context stream, synchronous.  The reference's train() is implied:
+ * the queries search everything added since creation or the last clear.
+ * The answers are the pairwise answers (cs_knn_match_line_descrip etc.) over the concatenation of every image added, in the same order:
+ *   - train_idx is the GLOBAL row in that concatenation (the reference's choice, not OpenCV's usual row within its image);
+ *   - img_idx is the image of the row as the reference's add() records it: an image of 0 codes followed by images starting at the same row
+ *     owns that row (std::map::insert keeps the first), so a later non-empty image's matches report the empty image's index, and that
+ *     index selects the mask;
+ *   - masks (NULL: none; else n_masks = the number of images, mask i at masks + i * n_query, one byte per query, 0 = skip) filter entries
+ *     after the selection: an entry survives when the mask of its image keeps its query.  match does not fall back to the next nearest code
+ *     when the nearest one's image masks the query: that query gets no match.  n_masks other than the number of images (or nonzero
+ *     without masks) is CS_ERR_INVALID_ARG.
+ * Where the reference is undefined this is defined:
+ *   - a query meets fewer than k codes, or none at all: fewer entries, no match (as the pairwise forms);
+ *   - an entry further than D = 128 bits away reports train_idx -1 and img_idx -1 (its trainIdx is never written there); with masks such
+ *     entries are dropped, as there is no image mask to consult;
+ *   - a second query after more add()s (the reference re-populates its hash with rows restarting at 0, and a second collection
+ *     radiusMatch runs with setK(0)): every query answers as the reference's first query after all the add()s since creation or clear().
+ * An empty collection or query set gives no entries; k = 0 gives none; k < 0 is CS_ERR_INVALID_ARG.
+ * Output layouts and the radius protocol are the pairwise ones: knn writes query i's n_per_query[i] entries at matches[i * k]; match writes
+ * its matches in query order, *n_matches of them (room for n_query); radius writes query i's entries at matches[match_offsets[i] ..
+ * match_offsets[i + 1]) and returns CS_ERR_CAPACITY with match_offsets (n_query + 1) filled when they exceed max_matches. */
+typedef struct cs_lbd_collection cs_lbd_collection;
+cs_lbd_collection *cs_lbd_collection_create(cs_ctx *ctx); /* NULL when ctx is NULL */
+void cs_lbd_collection_destroy(cs_lbd_collection *coll);
+int cs_lbd_collection_add(cs_lbd_collection *coll, const uint8_t *codes32, const int32_t *image_offsets, int n_images);
+int cs_lbd_collection_clear(cs_lbd_collection *coll);
+int cs_lbd_collection_size(const cs_lbd_collection *coll, int32_t *n_images, int64_t *n_codes);
+int cs_lbd_collection_match(cs_lbd_collection *coll, const uint8_t *query32, int n_query, const uint8_t *masks, int n_masks, cs_dmatch *matches,
+                            int32_t *n_matches);
+int cs_lbd_collection_knn_match(cs_lbd_collection *coll, const uint8_t *query32, int n_query, int k, const uint8_t *masks, int n_masks,
+                                cs_dmatch *matches, int32_t *n_per_query);
+int cs_lbd_collection_radius_match(cs_lbd_collection *coll, const uint8_t *query32, int n_query, float max_distance, const uint8_t *masks,
+                                   int n_masks, cs_dmatch *matches, int64_t max_matches, int64_t *match_offsets);
+
 /* tests: what the host side hands the descriptor kernel -- per key line {mid x, mid y, cos, sin, length, frame} (6 x 4 bytes) -- and the
  * two Gaussian weight tables F_g (63) and F_l (21) as floats (binary_descriptor.cpp:140-179).  Host-only, needs no context. */
 int cs_lbd_debug_prepare(const cs_keyline *keylines, int n, void *lines24, float *coef_g63, float *coef_l21);
