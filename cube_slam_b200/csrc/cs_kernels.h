@@ -11,21 +11,25 @@
  * L1 / shared split when it is idle.  75 % shared (a preference: a kernel that needs more shared memory still gets it).  H100, c3
  * headline with 12 batches in flight: 8.75 ms per step at 75 % shared, 9.06 with the driver's per-kernel choice. */
 #define CS_SMEM_CARVEOUT_PCT 75
-/* Function attributes are per device: `cs_first_on_device(flags)` is true the first time it runs on the current device (the flag word is
- * a bit per device ordinal, updated atomically: contexts on several devices / host threads may launch the same kernel). */
+/* Function attributes are per device: CS_ONCE_PER_DEVICE(body) runs body until it has completed once on the current device (the flag word
+ * is a bit per device ordinal: contexts on several devices / host threads may launch the same kernel).  The bit is set only AFTER the body
+ * has run, so a thread that finds it set knows the attribute is in place before its launch.  Threads that arrive together all run the body;
+ * every body sets constants, so running it twice does no harm.  (Setting the bit first would let a second thread skip the body and launch
+ * with more than 48 KB of dynamic shared memory before the first thread had raised the limit.) */
 #include <atomic>
-static inline bool cs_first_on_device(std::atomic<unsigned long long> &flags)
+static inline unsigned long long cs_device_bit()
 {
     int dev = 0;
     cudaGetDevice(&dev);
-    const unsigned long long bit = 1ull << (dev & 63);
-    return (flags.fetch_or(bit) & bit) == 0;
+    return 1ull << (dev & 63);
 }
 #define CS_ONCE_PER_DEVICE(...)                                    \
     do {                                                           \
         static std::atomic<unsigned long long> once_flags_{0};     \
-        if (cs_first_on_device(once_flags_)) {                     \
+        const unsigned long long once_bit_ = cs_device_bit();      \
+        if ((once_flags_.load() & once_bit_) == 0) {               \
             __VA_ARGS__;                                           \
+            once_flags_.fetch_or(once_bit_);                       \
         }                                                          \
     } while (0)
 /* let a kernel use as much dynamic shared memory as the device offers beyond its static allocation (the opt-in limit, 227 KB on H100) */

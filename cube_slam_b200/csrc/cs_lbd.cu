@@ -36,6 +36,9 @@
 
 #include "cs_internal.h"
 #include "cs_lbd_core.h"
+#if defined(__CUDACC__)
+#include "cs_kernels.h" /* CS_ONCE_PER_DEVICE */
+#endif
 
 namespace {
 

@@ -221,12 +221,16 @@ inline void launch_lbd_knn2(unsigned grid, cudaStream_t st, const uint4 *q_all, 
 {
     k_lbd_knn2<<<grid, 128, 0, st>>>(q_all, t_all, pair_of_query, t_off, n_queries, keys2);
 }
-/* sort_cap: keys of shared memory to reserve (a power of two, at most CS_LBD_KNN_MAX_TRAIN; 0 with keys == NULL) */
+/* sort_cap: keys of shared memory to reserve (a power of two, at most CS_LBD_KNN_MAX_TRAIN; 0 with keys == NULL).  The kernel's dynamic
+ * shared-memory limit is raised once per device to the most any launch asks for (CS_LBD_KNN_MAX_TRAIN keys, 128 KB), not to this launch's
+ * own size: the attribute belongs to the function on the device, shared by every context and host thread, so a limit lowered by one call
+ * could land between another thread's raise and its launch.  The limit is only a cap: occupancy still follows each launch's size. */
 inline void launch_lbd_match_sorted(unsigned grid, cudaStream_t st, unsigned sort_cap, const uint4 *q_all, const uint4 *t_all, const int32_t *pair_of_query,
                                     const int32_t *t_off, int n_queries, int max_dist, const long long *out_off, unsigned long long *keys, int32_t *counts)
 {
     const int smem = (int)(sort_cap * sizeof(unsigned long long));
-    if (smem > 48 * 1024) cudaFuncSetAttribute(k_lbd_match_sorted, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    CS_ONCE_PER_DEVICE(cudaFuncSetAttribute(k_lbd_match_sorted, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)(CS_LBD_KNN_MAX_TRAIN * sizeof(unsigned long long))));
     k_lbd_match_sorted<<<grid, CS_LBD_SORT_THREADS, smem, st>>>(q_all, t_all, pair_of_query, t_off, n_queries, max_dist, out_off, keys, counts);
 }
 #elif defined(CS_LBD_EMU_LAUNCH)

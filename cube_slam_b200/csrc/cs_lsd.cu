@@ -1325,17 +1325,6 @@ int ensure(cs_ctx *c, Buf &b, size_t bytes)
 
 inline int grid_for(int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, CS_SM_COUNT * 32); }
 
-/* raise a kernel's dynamic shared-memory limit when a launch needs more than it was last given (per device) */
-#define CS_LSD_SET_SMEM(kernel, bytes)                                                                  \
-    do {                                                                                                \
-        static size_t set_[64] = {};                                                                    \
-        const int dev_ = cs_ctx_device(c) & 63;                                                         \
-        if ((bytes) > set_[dev_]) {                                                                     \
-            cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(bytes));    \
-            set_[dev_] = (bytes);                                                                       \
-        }                                                                                               \
-    } while (0)
-
 /* k_lsd_front over n_frames frames (scaled == nullptr), or the debug instantiation over one frame: the scaled plane and the full modgrad plane */
 void lsd_front(cs_ctx *c, const uint8_t *d_img, int n_frames, int w, int h, int stride, int channels, int W, int H, double rho, double *modgrad,
                float *angf, uint4 *pix, double *scaled, int32_t *d_err)

@@ -165,7 +165,12 @@ int cs_detect_frames_batch(cs_ctx *ctx, const uint8_t *imgs, int n_frames, int w
                            const cs_line_params *line_params, const cs_cuboid_params *params, cs_cuboid_rec *out,
                            int32_t *out_counts);
 
-/* Device-resident variant used by the throughput benchmark: upload once, run many times, fetch. */
+/* Device-resident variant used by the throughput benchmark: upload once, run many times, fetch.
+ * Reuse of the caller's buffers: cs_batch_upload and cs_batch_upload_online copy imgs (and every table) on the context's stream and wait
+ * for that stream before they return, so imgs may be overwritten or freed as soon as the call returns, whether it is pageable or pinned
+ * host memory.  The wait also covers work still queued on this context (a cs_batch_run_async not yet fetched): an upload to a context
+ * with a batch in flight returns only when that batch has finished.  A pipeline that overlaps copies with kernels therefore keeps one
+ * context per batch in flight. */
 int cs_batch_upload(cs_ctx *ctx, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
                     const double *T_wc, const double *boxes, const int32_t *box_offsets, const double *lines,
                     const int32_t *line_offsets, const cs_cuboid_params *params);
