@@ -140,6 +140,9 @@ EXPORTS += MATCHER_EXPORTS
 COLLECTION_EXPORTS = ["cs_lbd_collection_create", "cs_lbd_collection_destroy", "cs_lbd_collection_add", "cs_lbd_collection_clear",
                       "cs_lbd_collection_size", "cs_lbd_collection_match", "cs_lbd_collection_knn_match", "cs_lbd_collection_radius_match"]
 EXPORTS += COLLECTION_EXPORTS
+# the LSD seed loop's defined-angle bit plane (cs_lsd.cu), bound the same way
+LSD_DEBUG_EXPORTS = ["cs_debug_lsd_defb"]
+EXPORTS += LSD_DEBUG_EXPORTS
 
 
 def load():
@@ -188,6 +191,8 @@ def load():
     L.cs_debug_lsd.argtypes = [vp, i, i32_p, d_p, d_p, d_p, i32_p, i32_p, f_p, i32_p, i]
     L.cs_debug_lsd_stats.argtypes = [vp, i32_p, i32_p, i]
     L.cs_debug_lsd_prof.argtypes = [vp, C.POINTER(C.c_uint64), i]
+    if hasattr(L, "cs_debug_lsd_defb"):
+        L.cs_debug_lsd_defb.argtypes = [vp, i, C.POINTER(C.c_uint32), i32_p]
     L.cs_debug_atan2.argtypes = [vp, d_p, d_p, d_p, i]
     L.cs_atan2_host.argtypes = [C.c_double, C.c_double]
     L.cs_atan2_host.restype = C.c_double
@@ -232,7 +237,7 @@ def load():
         L.cs_batch_upload_online_device.argtypes = [vp, df_p, d_p, d_p, i32_p, C.POINTER(LineParams), C.POINTER(CuboidParams)]
         L.cs_detect_lines_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), f_p, C.c_int32, i32_p]
     for name in EXPORTS:
-        if name in DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS and not hasattr(L, name):
+        if name in DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS + LSD_DEBUG_EXPORTS and not hasattr(L, name):
             continue
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("cs_abi_version",):

@@ -124,6 +124,7 @@ cudaStream_t cs_ctx_stream(cs_ctx *c) { return c->stream; }
 int cs_ctx_device(cs_ctx *c) { return c->device; }
 void **cs_ctx_lsd_slot(cs_ctx *c) { return &c->lsd_state; }
 int cs_ctx_seq_lines(cs_ctx *c) { return c->seq_lines; }
+int cs_ctx_profiling(cs_ctx *c) { return c->profiling ? 1 : 0; }
 int cs_ctx_use_tma(cs_ctx *c) { return c->use_tma ? 1 : 0; }
 void **cs_ctx_edl_slot(cs_ctx *c) { return &c->edl_state; }
 void **cs_ctx_lbd_slot(cs_ctx *c) { return &c->lbd_state; }

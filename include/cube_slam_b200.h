@@ -268,10 +268,12 @@ int cs_debug_lsd(cs_ctx *ctx, int frame, int32_t scaled_wh[2], double *scaled, d
  * that round 2 measured and removed); redo[f] = 1: the frame went through the one-warp-per-frame kernel, as every frame does now */
 int cs_debug_lsd_stats(cs_ctx *ctx, int32_t *stats4, int32_t *redo, int n_frames);
 /* clock64 cycles the seed-loop warps spent per phase since the last reset (diagnostics; tools/time_lines.py): {region_grow, region2rect,
- * refine, rectangle pixel counts, binomial tails (nfa), seeds grown, whole kernel summed over CTAs, region pixels, and eight more slots of
- * finer counters inside region_grow}.  Slots 3 and 4 read zero: the rectangle counts and binomial tails run in the validation phase
- * kernels, which keep no counters. */
+ * refine, raster scan for seeds (the seed loop outside the per-seed pipeline), used-map re-reads after a grow (a count), seeds grown, whole
+ * kernel summed over CTAs, region pixels, and eight unused slots}; only runs made while profiling is enabled (cs_set_profiling bit 0) count */
 int cs_debug_lsd_prof(cs_ctx *ctx, uint64_t *out16, int reset);
+/* the last LSD run's "angle defined" bit plane of one frame, as the seed loop scans it: bit x & 31 of word y * words_per_row + x / 32 of the
+ * scaled image, words_per_row = ceil(W / 32); bits holds H * words_per_row words; either pointer may be NULL */
+int cs_debug_lsd_defb(cs_ctx *ctx, int frame, uint32_t *bits, int32_t *words_per_row);
 /* same for the EDLines flavour (use_LSD = 0): EDLineDetector's maps (binary_descriptor.cpp:1617-1666: blurred image, dxImg_, dyImg_,
  * gImgWO_ / 4, dirImg_), the anchors in scan order as y * width + x, the edge map after smart routing, the segments before the length filter */
 int cs_debug_edlines(cs_ctx *ctx, int frame, uint8_t *blur, int16_t *dx, int16_t *dy, int16_t *g, uint8_t *dir, int32_t *anchors,

@@ -40,6 +40,12 @@ def main():
     flags = 128 if args.seq else 0
     ctx.set_profiling(1 | flags)
     ctx.upload_online(imgs, Ts, boxes, det.params(), cs.default_params())
+    try:
+        import subprocess
+        print("GPU:", subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                                     capture_output=True, text=True, timeout=30).stdout.strip(), flush=True)
+    except (OSError, subprocess.SubprocessError):
+        pass
     import ctypes as C
     prof = np.zeros(16, np.uint64)
     for r in range(args.reps):
@@ -51,8 +57,8 @@ def main():
         if args.flavour == "lsd":
             ctx.L.cs_debug_lsd_prof(ctx.h, prof.ctypes.data_as(C.POINTER(C.c_uint64)), 0)
             pf = prof.astype(np.float64) / args.frames
-            msg += " | Mcycles/frame: grow %.2f rect %.2f refine %.2f count %.2f nfa %.2f kernel %.2f, seeds grown/frame %.0f, region px/frame %.0f" % (
-                pf[0] / 1e6, pf[1] / 1e6, pf[2] / 1e6, pf[3] / 1e6, pf[4] / 1e6, pf[6] / 1e6, pf[5], pf[7])
+            msg += (" | Mcycles/frame: scan %.2f grow %.2f rect %.2f refine %.2f kernel %.2f, seeds grown/frame %.0f, region px/frame %.0f,"
+                    " used-map re-checks/frame %.0f") % (pf[3] / 1e6, pf[0] / 1e6, pf[1] / 1e6, pf[2] / 1e6, pf[6] / 1e6, pf[5], pf[7], pf[4])
         print(msg, flush=True)
 
 
