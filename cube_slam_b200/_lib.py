@@ -141,7 +141,7 @@ COLLECTION_EXPORTS = ["cs_lbd_collection_create", "cs_lbd_collection_destroy", "
                       "cs_lbd_collection_size", "cs_lbd_collection_match", "cs_lbd_collection_knn_match", "cs_lbd_collection_radius_match"]
 EXPORTS += COLLECTION_EXPORTS
 # the LSD seed loop's defined-angle bit plane (cs_lsd.cu), bound the same way
-LSD_DEBUG_EXPORTS = ["cs_debug_lsd_defb"]
+LSD_DEBUG_EXPORTS = ["cs_debug_lsd_defb", "cs_debug_lsd_occupancy"]
 EXPORTS += LSD_DEBUG_EXPORTS
 
 
@@ -193,6 +193,8 @@ def load():
     L.cs_debug_lsd_prof.argtypes = [vp, C.POINTER(C.c_uint64), i]
     if hasattr(L, "cs_debug_lsd_defb"):
         L.cs_debug_lsd_defb.argtypes = [vp, i, C.POINTER(C.c_uint32), i32_p]
+    if hasattr(L, "cs_debug_lsd_occupancy"):
+        L.cs_debug_lsd_occupancy.argtypes = [vp, i32_p]
     L.cs_debug_atan2.argtypes = [vp, d_p, d_p, d_p, i]
     L.cs_atan2_host.argtypes = [C.c_double, C.c_double]
     L.cs_atan2_host.restype = C.c_double

@@ -65,6 +65,7 @@
 
 #define LSD_CAND_CAP 2048    /* candidate rectangles per frame handed from the seed loop to the validation kernels, until a frame needs more */
 #define LSD_SEQ_SCAP 2048    /* region entries k_lsd_grow_seq keeps in shared memory (the rest spill to HBM; small, so that many frames share an SM) */
+#define LSD_SEQ_SMEM (LSD_SEQ_SCAP * 4 + 96 * 8) /* its dynamic shared memory: region list + staging of the ordered sums (SCAP even: 8-byte aligned) */
 #define LSD_HDR 8            /* ints of a candidate record header in the arena: n1, n2, has_line, x1 y1 x2 y2 (float bits), pad */
 
 namespace {
@@ -297,7 +298,7 @@ __global__ void __launch_bounds__(256) k_lsd_front(const __grid_constant__ CUten
 
 /* ---------------------------------------------------------------------------------------- the seed loop */
 /* cycle counters of the seed loop's phases (diagnostics, cs_debug_lsd_prof): grow, region2rect, refine, raster scan, used-map re-reads,
- * seeds grown, whole kernel, region pixels */
+ * seeds grown, whole kernel, region pixels, region lists past the shared-memory part */
 __device__ unsigned long long g_lsd_prof[16];
 /* only in the instantiation for a profiling context (cs_set_profiling bit 0, kProf): a run that is not being measured pays neither the
  * clock reads nor the atomics of thousands of warps on the same sixteen words */
@@ -306,6 +307,13 @@ __device__ unsigned long long g_lsd_prof[16];
     do {                                                                                           \
         if (kProf && (threadIdx.x & 31) == 0) atomicAdd(&g_lsd_prof[slot], (unsigned long long)(clock64() - prof_t0__)); \
     } while (0)
+
+/* k_lsd_grow_seq's dynamic shared memory (LSD_SEQ_SMEM): the first LSD_SEQ_SCAP entries of the region list (LsdReg), then 96 doubles
+ * that stage the addends of the ordered sums.  Named here rather than handed around as a pointer in LsdReg / LsdFrame: those structs go
+ * by reference to out-of-line functions, and a pointer that passes through them is a generic address, so every region-list read on the
+ * growth chain was a generic load (LD) instead of a shared-memory load (LDS). */
+extern __shared__ __align__(8) int s_seq[];
+__device__ __forceinline__ double *lsd_stage() { return reinterpret_cast<double *>(s_seq + LSD_SEQ_SCAP); }
 
 struct LsdFrame {
     int W, H;
@@ -325,23 +333,20 @@ struct LsdFrame {
         return ubits + y * WW + (x >> 5);
     }
     struct LsdSpan *span; /* k_lsd_val_count: room for five row-span records per warp (shared memory) */
-    double *stage;        /* k_lsd_grow_seq: 96 doubles of shared memory per warp (ordered sums) */
     const double *lgam; /* log_gamma of small integers (cs_nfa.cuh) */
     unsigned long long wmagic; /* ceil(2^40 / W): row of a pixel address without an integer division (exact for addresses < 2^20 .. 2^30 / W) */
-    __device__ __forceinline__ int row_of(int addr) const { return (int)(((unsigned long long)addr * wmagic) >> 40); }
+    __device__ __forceinline__ int row_of(int addr) const { return (int)(((unsigned long long)(unsigned)addr * wmagic) >> 40); }
 };
 
-/* the region list of the candidate a warp works on: the first `scap` entries in shared memory, the rest in HBM */
+/* the region list of the candidate a warp works on: the first LSD_SEQ_SCAP entries in shared memory (s_seq), the rest in HBM */
 struct LsdReg {
-    int *s;
     int *g;
-    int scap;
     int cap;
-    __device__ __forceinline__ int get(int i) const { return i < scap ? s[i] : __ldcg(g + i); }
+    __device__ __forceinline__ int get(int i) const { return i < LSD_SEQ_SCAP ? s_seq[i] : __ldcg(g + i); }
     __device__ __forceinline__ void put(int i, int v) const
     {
-        if (i < scap)
-            s[i] = v;
+        if (i < LSD_SEQ_SCAP)
+            s_seq[i] = v;
         else
             g[i] = v;
     }
@@ -558,12 +563,12 @@ __device__ void lsd_region_grow(const LsdFrame &F, const LsdReg &R, int base, in
 
 /* Sums over the region in the reference's order (the order decides the last bits of a double sum): 32 region points at a time, every lane
  * computes the addend(s) of ITS point -- the products round the same wherever they are computed -- and stages them in shared memory
- * (F.stage, 96 doubles per warp); then the additions run as one chain over the staged values, read as broadcasts. */
+ * (lsd_stage(), 96 doubles); then the additions run as one chain over the staged values, read as broadcasts. */
 /* lsd.cpp:690-784 */
 __device__ void lsd_region2rect(const LsdFrame &F, const LsdReg &R, int base, int reg_size, double reg_angle, double prec, double p, LsdRect &rec)
 {
     const int lane = threadIdx.x & 31;
-    double *st = F.stage;
+    double *st = lsd_stage();
     double x = 0, y = 0, sum = 0;
     for (int i0 = 0; i0 < reg_size; i0 += 32) {
         const int n = min(32, reg_size - i0);
@@ -962,8 +967,8 @@ __device__ void lsd_grow_candidate(const LsdFrame &F, const LsdReg &R, int s_add
                 if (lsd_dist(xc, yc, (double)rx, (double)ry) < rec.width) {
                     near = true;
                     const double ang_d = lsd_angle_diff_signed((double)F.angf[addr] * LSD_DEG2RAD, ang_c);
-                    F.stage[lane] = ang_d;
-                    F.stage[32 + lane] = ang_d * ang_d;
+                    lsd_stage()[lane] = ang_d;
+                    lsd_stage()[32 + lane] = ang_d * ang_d;
                 }
             }
             __syncwarp();
@@ -972,8 +977,8 @@ __device__ void lsd_grow_candidate(const LsdFrame &F, const LsdReg &R, int s_add
             while (todo) {
                 const int j = __ffs(todo) - 1;
                 todo &= todo - 1;
-                sum += F.stage[j];
-                s_sum += F.stage[32 + j];
+                sum += lsd_stage()[j];
+                s_sum += lsd_stage()[32 + j];
             }
         }
         for (int i = lane; i < reg_size; i += 32) {
@@ -1049,7 +1054,7 @@ struct LsdGrowArgs {
 
 /* The order-dependent half of the seed loop, one warp per frame (see the file header). */
 template <bool kProf>
-__global__ void __launch_bounds__(32, 21) k_lsd_grow_seq(LsdGrowArgs A, int scap)
+__global__ void __launch_bounds__(32, 21) k_lsd_grow_seq(LsdGrowArgs A)
 {
     const int f = blockIdx.x, lane = threadIdx.x;
     const size_t npx = (size_t)A.W * A.H;
@@ -1061,20 +1066,16 @@ __global__ void __launch_bounds__(32, 21) k_lsd_grow_seq(LsdGrowArgs A, int scap
     F.angf = A.angf + f * npx;
     F.modgrad = A.modgrad + f * npx;
     F.LOG_NT = A.LOG_NT;
-    extern __shared__ uint32_t s_seq[];
     const int WW = (A.W + 31) >> 5, n_words = WW * A.H;
     F.ubits = A.ubits + (size_t)f * n_words;
     F.WW = WW;
     F.span = nullptr;
-    F.stage = reinterpret_cast<double *>(s_seq + scap);
     F.lgam = A.lgam;
     F.wmagic = ((1ull << 40) + (unsigned long long)A.W - 1) / (unsigned long long)A.W;
     for (int i = lane; i < n_words; i += 32) F.ubits[i] = 0u;
     __syncwarp();
     LsdReg R;
-    R.s = (int *)s_seq; /* the first LSD_SEQ_SCAP region entries in shared memory, the rest in the (otherwise unused) record arena */
-    R.g = A.arena + (size_t)f * A.arena_cap;
-    R.scap = scap;
+    R.g = A.arena /* region entries past the first LSD_SEQ_SCAP (shared memory): the (otherwise unused) record arena */ + (size_t)f * A.arena_cap;
     R.cap = A.arena_cap;
     int n_cand = 0;
     /* Seeds in RASTER order: flsd walks its coorlist vector by index (lsd.cpp:478-480), and ll_angle fills that vector in scan order; the
@@ -1109,7 +1110,10 @@ __global__ void __launch_bounds__(32, 21) k_lsd_grow_seq(LsdGrowArgs A, int scap
             lsd_grow_candidate<kProf>(F, R, s_addr, A.min_reg_size, A.prec, A.p, n_all, has_rect, rec); /* arena_cap >= 2 W H: both passes fit */
             if (kProf) {
                 in_cand += clock64() - c0;
-                if (lane == 0) atomicAdd(&g_lsd_prof[4], 1ull);
+                if (lane == 0) {
+                    atomicAdd(&g_lsd_prof[4], 1ull);
+                    if (n_all > LSD_SEQ_SCAP) atomicAdd(&g_lsd_prof[8], 1ull);
+                }
             }
             __syncwarp(); /* the grow's used-map atomics are visible to every lane */
             u = wi < n_words ? __ldcg(F.ubits + wi) : 0u;
@@ -1206,7 +1210,6 @@ __global__ void __launch_bounds__(128, 5) k_lsd_val_count(LsdGrowArgs A, int rou
     F.ubits = nullptr;
     __shared__ LsdSpan s_span[4][5];
     F.span = s_span[threadIdx.x >> 5];
-    F.stage = nullptr;
     F.lgam = A.lgam;
     F.wmagic = 0;
     const int n = min(A.n_cand[f], A.cand_cap);
@@ -1464,11 +1467,11 @@ int lsd_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, i
     A.cand_line = (int32_t *)S.candline.p;
     A.cand_state = (LsdCandState *)S.candstate.p;
     A.err = d_err;
-    const size_t smem = (size_t)LSD_SEQ_SCAP * 4 + 96 * 8; /* region list + the staging of the ordered sums (LSD_SEQ_SCAP is even: 8-byte aligned) */
+    const size_t smem = LSD_SEQ_SMEM;
     if (cs_ctx_profiling(c))
-        k_lsd_grow_seq<true><<<n_frames, 32, smem, st>>>(A, LSD_SEQ_SCAP);
+        k_lsd_grow_seq<true><<<n_frames, 32, smem, st>>>(A);
     else
-        k_lsd_grow_seq<false><<<n_frames, 32, smem, st>>>(A, LSD_SEQ_SCAP);
+        k_lsd_grow_seq<false><<<n_frames, 32, smem, st>>>(A);
     /* 256 warps per frame: a warp per candidate for all but the densest frames */
     for (int round = 0; round < 6; round++) {
         k_lsd_val_count<<<dim3(64, n_frames), 128, 0, st>>>(A, round);
@@ -1691,7 +1694,7 @@ int cs_debug_lsd_defb(cs_ctx *c, int frame, uint32_t *bits, int32_t *words_per_r
 
 /* cycle counters of the seed loop's phases summed over every warp since the last reset (diagnostics): {region_grow, region2rect, refine,
  * raster scan for seeds (everything outside lsd_grow_candidate), used-map re-reads after a grow, candidates grown, whole kernel (per CTA),
- * region pixels of the first grows}. */
+ * region pixels of the first grows, seeds whose region list outgrew its shared-memory part}. */
 int cs_debug_lsd_prof(cs_ctx *c, uint64_t *out16, int reset)
 {
     if (!c) return CS_ERR_INVALID_ARG;
@@ -1703,6 +1706,33 @@ int cs_debug_lsd_prof(cs_ctx *c, uint64_t *out16, int reset)
         cudaMemcpyToSymbol(g_lsd_prof, z, 128);
     }
     return cudaGetLastError() == cudaSuccess ? CS_OK : cs_ctx_fail(c, CS_ERR_CUDA, "debug copy failed");
+}
+
+/* resources and residency of the seed loop and the front end, as the device reports them (tools/lsd_occupancy.py) */
+int cs_debug_lsd_occupancy(cs_ctx *c, int32_t *out14)
+{
+    if (!c || !out14) return CS_ERR_INVALID_ARG;
+    cudaSetDevice(cs_ctx_device(c));
+    struct {
+        const void *fn;
+        int threads, dyn_smem;
+    } const k[2] = {{(const void *)k_lsd_grow_seq<false>, 32, LSD_SEQ_SMEM}, {(const void *)k_lsd_front<true, false>, 256, 0}};
+    for (int i = 0; i < 2; i++) {
+        cudaFuncAttributes a;
+        int per_sm = 0;
+        if (cudaFuncGetAttributes(&a, k[i].fn) != cudaSuccess ||
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k[i].fn, k[i].threads, k[i].dyn_smem) != cudaSuccess)
+            return cs_ctx_fail(c, CS_ERR_CUDA, "LSD kernel attribute query failed: %s", cudaGetErrorString(cudaGetLastError()));
+        int32_t *o = out14 + 7 * i;
+        o[0] = a.numRegs;
+        o[1] = (int32_t)a.localSizeBytes;
+        o[2] = (int32_t)a.sharedSizeBytes;
+        o[3] = k[i].dyn_smem;
+        o[4] = k[i].threads;
+        o[5] = per_sm;
+        o[6] = a.preferredShmemCarveout;
+    }
+    return CS_OK;
 }
 
 /* kept for ABI stability (see the header): the seed loop runs one warp per frame with no speculative rounds, so stats4 reads zero and

@@ -269,8 +269,13 @@ int cs_debug_lsd(cs_ctx *ctx, int frame, int32_t scaled_wh[2], double *scaled, d
 int cs_debug_lsd_stats(cs_ctx *ctx, int32_t *stats4, int32_t *redo, int n_frames);
 /* clock64 cycles the seed-loop warps spent per phase since the last reset (diagnostics; tools/time_lines.py): {region_grow, region2rect,
  * refine, raster scan for seeds (the seed loop outside the per-seed pipeline), used-map re-reads after a grow (a count), seeds grown, whole
- * kernel summed over CTAs, region pixels, and eight unused slots}; only runs made while profiling is enabled (cs_set_profiling bit 0) count */
+ * kernel summed over CTAs, region pixels, seeds whose region list outgrew its shared-memory part (LSD_SEQ_SCAP entries), and seven unused
+ * slots}; only runs made while profiling is enabled (cs_set_profiling bit 0) count */
 int cs_debug_lsd_prof(cs_ctx *ctx, uint64_t *out16, int reset);
+/* resources of the LSD seed loop (k_lsd_grow_seq, out14[0..6]) and front end (k_lsd_front, out14[7..13]) on the context's device, each
+ * {registers per thread, local memory bytes per thread, static shared bytes, dynamic shared bytes per launch, threads per CTA, CTAs an SM
+ * holds at that launch configuration (cudaOccupancyMaxActiveBlocksPerMultiprocessor), preferred shared-memory carveout in percent} */
+int cs_debug_lsd_occupancy(cs_ctx *ctx, int32_t *out14);
 /* the last LSD run's "angle defined" bit plane of one frame, as the seed loop scans it: bit x & 31 of word y * words_per_row + x / 32 of the
  * scaled image, words_per_row = ceil(W / 32); bits holds H * words_per_row words; either pointer may be NULL */
 int cs_debug_lsd_defb(cs_ctx *ctx, int frame, uint32_t *bits, int32_t *words_per_row);

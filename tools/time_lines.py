@@ -58,7 +58,9 @@ def main():
             ctx.L.cs_debug_lsd_prof(ctx.h, prof.ctypes.data_as(C.POINTER(C.c_uint64)), 0)
             pf = prof.astype(np.float64) / args.frames
             msg += (" | Mcycles/frame: scan %.2f grow %.2f rect %.2f refine %.2f kernel %.2f, seeds grown/frame %.0f, region px/frame %.0f,"
-                    " used-map re-checks/frame %.0f") % (pf[3] / 1e6, pf[0] / 1e6, pf[1] / 1e6, pf[2] / 1e6, pf[6] / 1e6, pf[5], pf[7], pf[4])
+                    " used-map re-checks/frame %.0f, region lists past the shared-memory part (LSD_SEQ_SCAP entries) %d (%.3f %% of seeds grown)") % (
+                        pf[3] / 1e6, pf[0] / 1e6, pf[1] / 1e6, pf[2] / 1e6, pf[6] / 1e6, pf[5], pf[7], pf[4], int(prof[8]),
+                        100.0 * float(prof[8]) / max(float(prof[4]), 1.0))
         print(msg, flush=True)
 
 
