@@ -143,6 +143,10 @@ EXPORTS += COLLECTION_EXPORTS
 # the LSD seed loop's defined-angle bit plane (cs_lsd.cu), bound the same way
 LSD_DEBUG_EXPORTS = ["cs_debug_lsd_defb", "cs_debug_lsd_occupancy"]
 EXPORTS += LSD_DEBUG_EXPORTS
+# the line descriptor's two calls on frames already on the device (cs_ingest.cu), bound the same way: the host builds of cs_lbd.cu that the
+# CPU test suite compiles do not have them
+LBD_DEVICE_FRAME_EXPORTS = ["cs_detect_descrip_lines_batch_device", "cs_lbd_compute_batch_device"]
+EXPORTS += LBD_DEVICE_FRAME_EXPORTS
 
 
 def load():
@@ -238,8 +242,12 @@ def load():
         L.cs_batch_upload_device.argtypes = [vp, df_p, d_p, d_p, i32_p, d_p, i32_p, C.POINTER(CuboidParams)]
         L.cs_batch_upload_online_device.argtypes = [vp, df_p, d_p, d_p, i32_p, C.POINTER(LineParams), C.POINTER(CuboidParams)]
         L.cs_detect_lines_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), f_p, C.c_int32, i32_p]
+    if all(hasattr(L, n) for n in LBD_DEVICE_FRAME_EXPORTS):
+        df_p = C.POINTER(DeviceFrames)
+        L.cs_detect_descrip_lines_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), vp, u8_p, C.c_int32, i32_p]
+        L.cs_lbd_compute_batch_device.argtypes = [vp, df_p, vp, i32_p, u8_p, f_p]
     for name in EXPORTS:
-        if name in DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS + LSD_DEBUG_EXPORTS and not hasattr(L, name):
+        if name in DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS + LSD_DEBUG_EXPORTS + LBD_DEVICE_FRAME_EXPORTS and not hasattr(L, name):
             continue
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("cs_abi_version",):

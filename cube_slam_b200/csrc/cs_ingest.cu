@@ -1,6 +1,6 @@
 /*
- * cs_ingest.cu -- frames that are already in GPU memory: the descriptor check, the layout kernel k_ingest_frames, and the three entry points
- * that take a cs_device_frames (include/cube_slam_b200.h).
+ * cs_ingest.cu -- frames that are already in GPU memory: the descriptor check, the layout kernel k_ingest_frames, and the entry points that
+ * take a cs_device_frames (include/cube_slam_b200.h): the batch uploads, line detection, and the line descriptor's two calls.
  *
  * Every consumer of a batch's frames (k_bgr2gray_flat, k_lsd_front, k_ed_front) reads packed rows, BGR or gray, pitch width * channels.
  * A device view of any strides is brought into that layout once, on the context stream, so that everything downstream runs exactly the code
@@ -258,6 +258,45 @@ int cs_detect_lines_batch_device(cs_ctx *c, const cs_device_frames *frames, cons
     if (!buf) return CS_ERR_CUDA; /* the allocation's failure is already the context's message */
     if ((rc = ingest(c, frames, buf))) return rc;
     return cs_detect_lines_run(c, buf, true, F, W, H, W * ch, ch, params, lines_xyxy, max_lines_per_frame, n_lines);
+}
+
+/* cs_detect_descrip_lines_batch on device frames: the detector runs on its own buffer, then the host form's body (cs_lbd.cu) */
+int cs_detect_descrip_lines_batch_device(cs_ctx *c, const cs_device_frames *frames, const cs_line_params *params, cs_keyline *keylines,
+                                         uint8_t *desc32, int32_t max_lines_per_frame, int32_t *n_lines)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    if (!params || !keylines || !desc32 || !n_lines || max_lines_per_frame <= 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
+    if (params->numoctaves < 1) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "numoctaves must be at least 1"); /* as cs_detect_descrip_lines_batch */
+    int rc;
+    if ((rc = check_on_ctx(c, frames))) return rc;
+    cudaSetDevice(cs_ctx_device(c));
+    const int F = frames->n_frames, W = frames->width, H = frames->height, ch = frames->channels, cap = max_lines_per_frame;
+    const size_t bytes = (size_t)F * H * W * ch;
+    uint8_t *buf = params->use_LSD ? cs_lsd_frame_buffer(c, bytes) : cs_edl_frame_buffer(c, bytes);
+    if (!buf) return CS_ERR_CUDA;
+    if ((rc = ingest(c, frames, buf))) return rc;
+    CsDetectedLines d;
+    if (params->use_LSD) {
+        if ((rc = cs_lsd_run_sync(c, buf, true, F, W, H, W * ch, ch, params->line_length_thres, cap, &d.lines, &d.counts, &d.lsd_frames))) return rc;
+    } else if ((rc = cs_edl_run_keylines(c, buf, true, F, W, H, W * ch, ch, params->line_length_thres, cap, &d.lines, &d.counts, &d.extra, &d.dx, &d.dy)))
+        return rc;
+    return cs_lbd_describe_detected(c, d, params->use_LSD != 0, F, W, H, W * ch, ch, keylines, desc32, cap, n_lines);
+}
+
+/* cs_lbd_compute_batch on device frames: the frames go to the EDLines buffer, whose front end makes the descriptor's Sobel maps */
+int cs_lbd_compute_batch_device(cs_ctx *c, const cs_device_frames *frames, const cs_keyline *keylines, const int32_t *keyline_offsets, uint8_t *desc32,
+                                float *desc72)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    int rc, n = 0;
+    if ((rc = check_on_ctx(c, frames))) return rc;
+    if ((rc = cs_lbd_check_given(c, frames->n_frames, keylines, keyline_offsets, desc32, &n)) || n == 0) return rc;
+    cudaSetDevice(cs_ctx_device(c));
+    const int F = frames->n_frames, W = frames->width, H = frames->height, ch = frames->channels;
+    uint8_t *buf = cs_edl_frame_buffer(c, (size_t)F * H * W * ch);
+    if (!buf) return CS_ERR_CUDA;
+    if ((rc = ingest(c, frames, buf))) return rc;
+    return cs_lbd_compute_run(c, buf, true, F, W, H, W * ch, ch, keylines, keyline_offsets, desc32, desc72);
 }
 
 } /* extern "C" */

@@ -97,6 +97,9 @@ int cs_edl_sobel_maps(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n
 /* LSD flavour of detect_filter_lines from host frames (the body of cs_detect_lines_batch's LSD branch): filtered segments + counts in HBM */
 int cs_lsd_run_host(cs_ctx *c, const uint8_t *imgs, int n_frames, int w, int h, int stride, int channels, float line_length_thres, int cap,
                     const float **d_lines, const int32_t **d_counts, const uint8_t **d_frames);
+/* the same synchronous run on host frames or on frames already in the LSD frame buffer; d_frames: the frames the run read, in HBM */
+int cs_lsd_run_sync(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int w, int h, int stride, int channels, float line_length_thres,
+                    int cap, const float **d_lines, const int32_t **d_counts, const uint8_t **d_frames);
 /* The line detectors' error words: 16 bytes in HBM per workspace, cleared at the start of every run (and of cs_edl_sobel_maps), set by
  * their kernels.  LSD: [0] 4 = a frame had more candidate rectangles than the hand-off buffer holds ([1]: the largest such count, [2]: the
  * buffer's size per frame), 8 = a TMA tile copy of the front end did not complete.  EDLines: [0] 1 = more anchors in a frame than
@@ -135,5 +138,22 @@ uint8_t *cs_edl_frame_buffer(cs_ctx *c, size_t bytes);
 int cs_detect_lines_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int width, int height, int stride, int channels,
                         const cs_line_params *params, float *lines_xyxy, int32_t max_lines_per_frame, int32_t *n_lines);
 void cs_lbd_destroy(void *state);           /* called from cs_destroy */
+/* what a synchronous detector run of the descriptor path leaves in HBM: the kept segments and their counts (cap per frame); EDLines: the
+ * {direction, numOfPixels} pairs and the Sobel maps the descriptor reads; LSD: the frames the detector read, for the Sobel maps */
+struct CsDetectedLines {
+    const float *lines = nullptr, *extra = nullptr;
+    const int32_t *counts = nullptr;
+    const int16_t *dx = nullptr, *dy = nullptr;
+    const uint8_t *lsd_frames = nullptr;
+};
+/* the body of cs_detect_descrip_lines_batch after detection (cs_lbd.cu): key lines filled on the host, descriptors, the per-frame slots;
+ * `stride` is the row pitch of d.lsd_frames */
+int cs_lbd_describe_detected(cs_ctx *c, const CsDetectedLines &d, bool use_LSD, int n_frames, int width, int height, int stride, int channels,
+                             cs_keyline *keylines, uint8_t *desc32, int32_t max_lines_per_frame, int32_t *n_lines);
+/* cs_lbd_compute_batch's key-line arguments: the CSR checked, *n its total; 0 = nothing to describe (no output touched) */
+int cs_lbd_check_given(cs_ctx *c, int n_frames, const cs_keyline *keylines, const int32_t *keyline_offsets, const uint8_t *desc32, int *n);
+/* the body of cs_lbd_compute_batch after its checks, on host frames or on frames already on the device (packed rows of `stride` bytes) */
+int cs_lbd_compute_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int width, int height, int stride, int channels,
+                       const cs_keyline *keylines, const int32_t *keyline_offsets, uint8_t *desc32, float *desc72);
 
 #endif

@@ -290,25 +290,89 @@ int cs_lbd_debug_prepare(const cs_keyline *keylines, int n, void *lines24, float
     return CS_OK;
 }
 
+}  // extern "C"
+
+/* ---- shared by the host-frame entry points below and their device-frame forms (cs_ingest.cu) */
+int cs_lbd_check_given(cs_ctx *c, int n_frames, const cs_keyline *keylines, const int32_t *keyline_offsets, const uint8_t *desc32, int *n)
+{
+    *n = 0;
+    if (!keyline_offsets || keyline_offsets[0] != 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "keyline_offsets must start at 0");
+    for (int f = 0; f < n_frames; f++)
+        if (keyline_offsets[f + 1] < keyline_offsets[f]) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "keyline_offsets must not decrease");
+    if (keyline_offsets[n_frames] == 0) return CS_OK; /* "Error: keypoint list is empty": descriptors left as they are (:622-626) */
+    if (!keylines || !desc32) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null key lines or output");
+    *n = keyline_offsets[n_frames];
+    return CS_OK;
+}
+
+int cs_lbd_compute_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int width, int height, int stride, int channels,
+                       const cs_keyline *keylines, const int32_t *keyline_offsets, uint8_t *desc32, float *desc72)
+{
+    cudaSetDevice(cs_ctx_device(c));
+    std::vector<CsLbdLine> lines((size_t)keyline_offsets[n_frames]);
+    for (int f = 0; f < n_frames; f++)
+        for (int i = keyline_offsets[f]; i < keyline_offsets[f + 1]; i++) lbd_prepare(keylines[i], f, lines[i]);
+    const int16_t *d_dx = nullptr, *d_dy = nullptr;
+    int rc;
+    if ((rc = cs_edl_sobel_maps(c, imgs, imgs_on_device, n_frames, width, height, stride, channels, &d_dx, &d_dy))) return rc;
+    return describe(c, *state_of(c), lines, d_dx, d_dy, width, height, desc32, desc72);
+}
+
+int cs_lbd_describe_detected(cs_ctx *c, const CsDetectedLines &d, bool use_LSD, int n_frames, int width, int height, int stride, int channels,
+                             cs_keyline *keylines, uint8_t *desc32, int32_t max_lines_per_frame, int32_t *n_lines)
+{
+    cudaStream_t st = cs_ctx_stream(c);
+    const int cap = max_lines_per_frame;
+    std::vector<int32_t> cnt((size_t)n_frames);
+    std::vector<float> seg((size_t)n_frames * cap * 4), extra(d.extra ? (size_t)n_frames * cap * 2 : 0);
+    if (cudaMemcpyAsync(cnt.data(), d.counts, (size_t)n_frames * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaMemcpyAsync(seg.data(), d.lines, seg.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        (d.extra && cudaMemcpyAsync(extra.data(), d.extra, extra.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
+        cudaStreamSynchronize(st) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "line result copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+    /* the KeyLine fill of the two detectors (LSDDetector.cpp:226-250; binary_descriptor.cpp:526-545) for the kept lines */
+    std::vector<CsLbdLine> lines;
+    std::vector<int32_t> first((size_t)n_frames + 1, 0);
+    for (int f = 0; f < n_frames; f++) {
+        if (cnt[f] > cap) return cs_ctx_fail(c, CS_ERR_CAPACITY, "frame %d: %d segments exceed max_lines_per_frame", f, cnt[f]);
+        n_lines[f] = cnt[f];
+        first[f + 1] = first[f] + cnt[f];
+        for (int k = 0; k < cnt[f]; k++) {
+            const float *e = &seg[((size_t)f * cap + k) * 4];
+            cs_keyline &kl = keylines[(size_t)f * cap + k];
+            if (use_LSD)
+                keyline_from_lsd_row(e, width, height, k, kl);
+            else
+                keyline_from_edl_row(e, &extra[((size_t)f * cap + k) * 2], width, height, k, kl);
+            CsLbdLine L;
+            lbd_prepare(kl, f, L);
+            lines.push_back(L);
+        }
+    }
+    /* computeImpl returns before computeSobel when there is no key line (binary_descriptor.cpp:617-622), and so does this */
+    if (lines.empty()) return CS_OK;
+    const int16_t *d_dx = d.dx, *d_dy = d.dy;
+    int rc;
+    if (d.lsd_frames && (rc = cs_edl_sobel_maps(c, d.lsd_frames, true, n_frames, width, height, stride, channels, &d_dx, &d_dy))) return rc;
+    /* descriptors come back line after line; hand each frame's rows to its slot */
+    std::vector<uint8_t> packed(lines.size() * CS_LBD_BYTES);
+    if ((rc = describe(c, *state_of(c), lines, d_dx, d_dy, width, height, packed.data(), nullptr))) return rc;
+    for (int f = 0; f < n_frames; f++)
+        if (cnt[f]) memcpy(desc32 + (size_t)f * cap * CS_LBD_BYTES, packed.data() + (size_t)first[f] * CS_LBD_BYTES, (size_t)cnt[f] * CS_LBD_BYTES);
+    return CS_OK;
+}
+
+extern "C" {
+
 int cs_lbd_compute_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels, const cs_keyline *keylines,
                          const int32_t *keyline_offsets, uint8_t *desc32, float *desc72)
 {
     if (!c) return CS_ERR_INVALID_ARG;
     int rc = check_image_args(c, imgs, n_frames, width, height, stride, channels);
     if (rc) return rc;
-    if (!keyline_offsets || keyline_offsets[0] != 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "keyline_offsets must start at 0");
-    for (int f = 0; f < n_frames; f++)
-        if (keyline_offsets[f + 1] < keyline_offsets[f]) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "keyline_offsets must not decrease");
-    const int n = keyline_offsets[n_frames];
-    if (n == 0) return CS_OK; /* "Error: keypoint list is empty": descriptors left as they are (:622-626) */
-    if (!keylines || !desc32) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null key lines or output");
-    cudaSetDevice(cs_ctx_device(c));
-    std::vector<CsLbdLine> lines((size_t)n);
-    for (int f = 0; f < n_frames; f++)
-        for (int i = keyline_offsets[f]; i < keyline_offsets[f + 1]; i++) lbd_prepare(keylines[i], f, lines[i]);
-    const int16_t *d_dx = nullptr, *d_dy = nullptr;
-    if ((rc = cs_edl_sobel_maps(c, imgs, false, n_frames, width, height, stride, channels, &d_dx, &d_dy))) return rc;
-    return describe(c, *state_of(c), lines, d_dx, d_dy, width, height, desc32, desc72);
+    int n = 0;
+    if ((rc = cs_lbd_check_given(c, n_frames, keylines, keyline_offsets, desc32, &n)) || n == 0) return rc;
+    return cs_lbd_compute_run(c, imgs, false, n_frames, width, height, stride, channels, keylines, keyline_offsets, desc32, desc72);
 }
 
 int cs_lbd_compute(cs_ctx *c, const uint8_t *img, int width, int height, int stride, int channels, const cs_keyline *keylines, int n, uint8_t *desc32,
@@ -330,53 +394,15 @@ int cs_detect_descrip_lines_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, 
     /* more octaves: both overloads of detect_descrip_lines keep octave 0 only (:239,266), whose lines and Sobel maps do not depend on the others */
     if (params->numoctaves < 1) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "numoctaves must be at least 1");
     cudaSetDevice(cs_ctx_device(c));
-    cudaStream_t st = cs_ctx_stream(c);
     const int cap = max_lines_per_frame;
-    const float *d_lines = nullptr, *d_extra = nullptr;
-    const int32_t *d_counts = nullptr;
-    const int16_t *d_dx = nullptr, *d_dy = nullptr;
-    const uint8_t *d_lsd_frames = nullptr; /* LSD: the detector's copy of the frames, for the Sobel maps once the key lines are known */
+    CsDetectedLines d; /* LSD: d.lsd_frames is the detector's copy of the frames, for the Sobel maps once the key lines are known */
     if (params->use_LSD) {
-        if ((rc = cs_lsd_run_host(c, imgs, n_frames, width, height, stride, channels, params->line_length_thres, cap, &d_lines, &d_counts, &d_lsd_frames)))
+        if ((rc = cs_lsd_run_host(c, imgs, n_frames, width, height, stride, channels, params->line_length_thres, cap, &d.lines, &d.counts, &d.lsd_frames)))
             return rc;
-    } else if ((rc = cs_edl_run_keylines(c, imgs, false, n_frames, width, height, stride, channels, params->line_length_thres, cap, &d_lines, &d_counts, &d_extra,
-                                         &d_dx, &d_dy)))
+    } else if ((rc = cs_edl_run_keylines(c, imgs, false, n_frames, width, height, stride, channels, params->line_length_thres, cap, &d.lines, &d.counts, &d.extra,
+                                         &d.dx, &d.dy)))
         return rc;
-    std::vector<int32_t> cnt((size_t)n_frames);
-    std::vector<float> seg((size_t)n_frames * cap * 4), extra(d_extra ? (size_t)n_frames * cap * 2 : 0);
-    if (cudaMemcpyAsync(cnt.data(), d_counts, (size_t)n_frames * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaMemcpyAsync(seg.data(), d_lines, seg.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        (d_extra && cudaMemcpyAsync(extra.data(), d_extra, extra.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
-        cudaStreamSynchronize(st) != cudaSuccess)
-        return cs_ctx_fail(c, CS_ERR_CUDA, "line result copy failed: %s", cudaGetErrorString(cudaGetLastError()));
-    /* the KeyLine fill of the two detectors (LSDDetector.cpp:226-250; binary_descriptor.cpp:526-545) for the kept lines */
-    std::vector<CsLbdLine> lines;
-    std::vector<int32_t> first((size_t)n_frames + 1, 0);
-    for (int f = 0; f < n_frames; f++) {
-        if (cnt[f] > cap) return cs_ctx_fail(c, CS_ERR_CAPACITY, "frame %d: %d segments exceed max_lines_per_frame", f, cnt[f]);
-        n_lines[f] = cnt[f];
-        first[f + 1] = first[f] + cnt[f];
-        for (int k = 0; k < cnt[f]; k++) {
-            const float *e = &seg[((size_t)f * cap + k) * 4];
-            cs_keyline &kl = keylines[(size_t)f * cap + k];
-            if (params->use_LSD)
-                keyline_from_lsd_row(e, width, height, k, kl);
-            else
-                keyline_from_edl_row(e, &extra[((size_t)f * cap + k) * 2], width, height, k, kl);
-            CsLbdLine L;
-            lbd_prepare(kl, f, L);
-            lines.push_back(L);
-        }
-    }
-    /* computeImpl returns before computeSobel when there is no key line (binary_descriptor.cpp:617-622), and so does this */
-    if (lines.empty()) return CS_OK;
-    if (d_lsd_frames && (rc = cs_edl_sobel_maps(c, d_lsd_frames, true, n_frames, width, height, stride, channels, &d_dx, &d_dy))) return rc;
-    /* descriptors come back line after line; hand each frame's rows to its slot */
-    std::vector<uint8_t> packed(lines.size() * CS_LBD_BYTES);
-    if ((rc = describe(c, *state_of(c), lines, d_dx, d_dy, width, height, packed.data(), nullptr))) return rc;
-    for (int f = 0; f < n_frames; f++)
-        if (cnt[f]) memcpy(desc32 + (size_t)f * cap * CS_LBD_BYTES, packed.data() + (size_t)first[f] * CS_LBD_BYTES, (size_t)cnt[f] * CS_LBD_BYTES);
-    return CS_OK;
+    return cs_lbd_describe_detected(c, d, params->use_LSD != 0, n_frames, width, height, stride, channels, keylines, desc32, cap, n_lines);
 }
 
 int cs_detect_descrip_lines(cs_ctx *c, const uint8_t *img, int width, int height, int stride, int channels, const cs_line_params *params, cs_keyline *keylines,

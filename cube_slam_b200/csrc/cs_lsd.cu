@@ -1522,15 +1522,22 @@ int cs_lsd_run_device(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int w, int
     return CS_OK;
 }
 
-/* host frames in, results stay in HBM (the synchronous descriptor path, cs_lbd.cu): waits for the run and reads its error word back; a
- * candidate overflow grows the buffer and runs once more */
+/* host frames in, results stay in HBM (the synchronous descriptor path, cs_lbd.cu) */
 int cs_lsd_run_host(cs_ctx *c, const uint8_t *imgs, int n_frames, int w, int h, int stride, int channels, float line_length_thres, int cap,
                     const float **d_lines, const int32_t **d_counts, const uint8_t **d_frames)
+{
+    return cs_lsd_run_sync(c, imgs, false, n_frames, w, h, stride, channels, line_length_thres, cap, d_lines, d_counts, d_frames);
+}
+
+/* waits for the run and reads its error word back; a candidate overflow grows the buffer and runs once more, on the same frames: host
+ * frames are copied in again, device frames (the LSD frame buffer, cs_ingest.cu) are still where they were */
+int cs_lsd_run_sync(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int w, int h, int stride, int channels, float line_length_thres,
+                    int cap, const float **d_lines, const int32_t **d_counts, const uint8_t **d_frames)
 {
     LsdState *S = state_of(c);
     cudaStream_t st = cs_ctx_stream(c);
     for (int pass = 0;; pass++) {
-        int rc = lsd_run(c, imgs, false, n_frames, w, h, stride, channels, line_length_thres, cap, *S);
+        int rc = lsd_run(c, imgs, imgs_on_device, n_frames, w, h, stride, channels, line_length_thres, cap, *S);
         if (rc) return rc;
         int32_t err[4] = {0, 0, 0, 0};
         if (cudaMemcpyAsync(err, S->err.p, sizeof err, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
@@ -1541,7 +1548,7 @@ int cs_lsd_run_host(cs_ctx *c, const uint8_t *imgs, int n_frames, int w, int h, 
     }
     *d_lines = (const float *)S->out.p;
     *d_counts = (const int32_t *)S->nout.p;
-    *d_frames = (const uint8_t *)S->img.p; /* the frames as uploaded (same stride), still in HBM */
+    *d_frames = imgs_on_device ? imgs : (const uint8_t *)S->img.p; /* the frames the run read (same stride), still in HBM */
     return CS_OK;
 }
 

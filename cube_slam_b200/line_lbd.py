@@ -5,7 +5,8 @@ detect_filter_lines(img) -> n x 4 float32 [x1 y1 x2 y2]: what the reference writ
 detect_descrip_lines_octaves, match_line_descrip; :191-198,224-356) return numpy arrays: key lines as records of `_lib.KEYLINE_DTYPE`
 (the KeyLine fields, octave 0), descriptors as n x 32 uint8 (the CV_8UC1 matrix), matches as records of `_lib.DMATCH_DTYPE` (cv::DMatch).
 `line_lbd_detect.bdm` is the class's BinaryDescriptorMatcher (line_lbd_allclass.h:37): pairwise match, knnMatch and radiusMatch on the GPU,
-and the collection forms (add / train / clear, then match / knnMatch / radiusMatch without a train matrix) against codes kept on the GPU."""
+and the collection forms (add / train / clear, then match / knnMatch / radiusMatch without a train matrix) against codes kept on the GPU.
+detect_filter_lines_device, detect_descrip_lines_device and compute_descriptors_device take frames that are already in GPU memory."""
 import ctypes as C
 import math
 import numbers
@@ -439,7 +440,30 @@ class line_lbd_detect(object):
             kl, desc = self.detect_descrip_lines_batch(np.asarray(gray_img)[None], cap)[0]
         finally:
             self.line_length_thres = keep
-        return np.stack([kl["start_x"], kl["start_y"], kl["end_x"], kl["end_y"]], 1).astype(np.float32).reshape(-1, 4), desc
+        return self._mat_rows(kl), desc
+
+    @staticmethod
+    def _mat_rows(kl):
+        """the Mat overload's lines: n x 4 float32 [start x, start y, end x, end y] of the key lines"""
+        return np.stack([kl["start_x"], kl["start_y"], kl["end_x"], kl["end_y"]], 1).astype(np.float32).reshape(-1, 4)
+
+    def detect_descrip_lines_device(self, frames, order="bgr", cap=4096, stream=None, as_mat=False):
+        """detect_descrip_lines_batch on frames already on the GPU -> [(key lines, n x 32 uint8 descriptors)] per frame, the same values the
+        host form returns for the same pixels.  frames, order and stream as detect_filter_lines_device: any object with
+        __cuda_array_interface__, uint8, (N, H, W, 3) or (N, H, W), any strides.  as_mat: the cv::Mat overload of every frame, as
+        detect_descrip_lines(..., as_mat=True) -- no length filter, lines as n x 4 float32."""
+        fr = _lib.device_frames(frames, order, stream)
+        F = fr.n_frames
+        kl = np.zeros((F, cap), _lib.KEYLINE_DTYPE)
+        desc = np.zeros((F, cap, 32), np.uint8)
+        n = np.zeros(F, np.int32)
+        p = self.params()
+        if as_mat:
+            p.line_length_thres = -1.0      # lineLength > -1: every octave-0 line, as the Mat overload keeps them
+        self._ctx.check(self._ctx.L.cs_detect_descrip_lines_batch_device(self._ctx.h, C.byref(fr), C.byref(p), kl.ctypes.data,
+                                                                         _lib.ptr(desc, C.c_uint8), cap, _lib.ptr(n, C.c_int32)))
+        out = [(kl[f, :n[f]].copy(), desc[f, :n[f]].copy()) for f in range(F)]
+        return [(self._mat_rows(k), d) for k, d in out] if as_mat else out
 
     def detect_descrip_lines_octaves(self, gray_img, cap=8192):
         """detect_descrip_lines_octaves (:285-339) for the one octave the class is built with: the kept key lines with start x <= end x
@@ -474,6 +498,25 @@ class line_lbd_detect(object):
         self._ctx.check(self._ctx.L.cs_lbd_compute(self._ctx.h, imgs.ctypes.data, W, H, W * ch, ch, kl.ctypes.data, len(kl), _lib.ptr(desc, C.c_uint8),
                                                    _lib.ptr(fdesc, C.c_float) if want_float else None))
         return (desc, fdesc) if want_float else desc
+
+    def compute_descriptors_device(self, frames, keylines_per_frame, want_float=False, order="bgr", stream=None):
+        """lbd->compute on frames already on the GPU (frames, order, stream as detect_filter_lines_device), frame f with the key lines
+        keylines_per_frame[f] (records of _lib.KEYLINE_DTYPE, any count including 0) -> per frame the n x 32 uint8 descriptors, or
+        (n x 32 uint8, n x 72 float32) with want_float."""
+        fr = _lib.device_frames(frames, order, stream)
+        kls = [np.ascontiguousarray(k, _lib.KEYLINE_DTYPE).reshape(-1) for k in keylines_per_frame]
+        if len(kls) != fr.n_frames:
+            raise CubeSlamError("one key-line array per frame: %d for %d frames" % (len(kls), fr.n_frames))
+        off = np.concatenate([[0], np.cumsum([len(k) for k in kls])]).astype(np.int32)
+        n = int(off[-1])
+        kl = np.ascontiguousarray(np.concatenate(kls)) if n else np.zeros(1, _lib.KEYLINE_DTYPE)
+        desc = np.zeros((max(n, 1), 32), np.uint8)
+        fdesc = np.zeros((max(n, 1), 72), np.float32) if want_float else None
+        self._ctx.check(self._ctx.L.cs_lbd_compute_batch_device(self._ctx.h, C.byref(fr), kl.ctypes.data, _lib.ptr(off, C.c_int32),
+                                                                _lib.ptr(desc, C.c_uint8), _lib.ptr(fdesc, C.c_float) if want_float else None))
+        if want_float:
+            return [(desc[off[f]:off[f + 1]].copy(), fdesc[off[f]:off[f + 1]].copy()) for f in range(fr.n_frames)]
+        return [desc[off[f]:off[f + 1]].copy() for f in range(fr.n_frames)]
 
     def get_line_descriptors(self, gray_img, linesmat_src):
         """get_line_descriptors(gray_img, linesmat_src, line_descrips) (:191-198): descriptors of given n x 4 lines.  The reference builds

@@ -212,6 +212,16 @@ int cs_batch_upload_online_device(cs_ctx *ctx, const cs_device_frames *frames, c
  * uploaded to the context reads from.  Synchronous, like the host form. */
 int cs_detect_lines_batch_device(cs_ctx *ctx, const cs_device_frames *frames, const cs_line_params *params, float *lines_xyxy,
                                  int32_t max_lines_per_frame, int32_t *n_lines /* n_frames */);
+/* cs_detect_descrip_lines_batch (below) on device frames: the same outputs -- host key lines, host 32-byte descriptors, frame f's slots at
+ * f * max_lines_per_frame -- the same checks (numoctaves >= 1, capacity) and the same error statuses and messages.  The frames go to the
+ * detector's own buffer (LSD or EDLines, after use_LSD), as in cs_detect_lines_batch_device.  Synchronous. */
+struct cs_keyline; /* defined with the line descriptors below */
+int cs_detect_descrip_lines_batch_device(cs_ctx *ctx, const cs_device_frames *frames, const cs_line_params *params, struct cs_keyline *keylines,
+                                         uint8_t *desc32, int32_t max_lines_per_frame, int32_t *n_lines /* n_frames */);
+/* cs_lbd_compute_batch (below) on device frames: the key lines and their CSR stay host buffers, desc72 is optional.  With no key line at all
+ * it returns CS_OK after the descriptor check, as the host form does.  The frames go to the EDLines detector's buffer.  Synchronous. */
+int cs_lbd_compute_batch_device(cs_ctx *ctx, const cs_device_frames *frames, const struct cs_keyline *keylines,
+                                const int32_t *keyline_offsets /* n_frames + 1 */, uint8_t *desc32, float *desc72);
 
 int cs_batch_run(cs_ctx *ctx);                       /* host-side sampling tables + every kernel; synchronous */
 int cs_batch_run_async(cs_ctx *ctx);                 /* same, returns after enqueueing on the context stream */
