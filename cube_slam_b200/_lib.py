@@ -143,6 +143,10 @@ EXPORTS += COLLECTION_EXPORTS
 # the LSD seed loop's defined-angle bit plane (cs_lsd.cu), bound the same way
 LSD_DEBUG_EXPORTS = ["cs_debug_lsd_defb", "cs_debug_lsd_occupancy"]
 EXPORTS += LSD_DEBUG_EXPORTS
+# the line detectors' NFA on given (n, k, p) (cs_debug_math.cu), bound the same way: the host build of cs_context.cu that the CPU test suite
+# compiles does not have it
+NFA_DEBUG_EXPORTS = ["cs_debug_nfa"]
+EXPORTS += NFA_DEBUG_EXPORTS
 # the line descriptor's two calls on frames already on the device (cs_ingest.cu), bound the same way: the host builds of cs_lbd.cu that the
 # CPU test suite compiles do not have them
 LBD_DEVICE_FRAME_EXPORTS = ["cs_detect_descrip_lines_batch_device", "cs_lbd_compute_batch_device"]
@@ -202,6 +206,8 @@ def load():
     L.cs_debug_atan2.argtypes = [vp, d_p, d_p, d_p, i]
     L.cs_atan2_host.argtypes = [C.c_double, C.c_double]
     L.cs_atan2_host.restype = C.c_double
+    if hasattr(L, "cs_debug_nfa"):
+        L.cs_debug_nfa.argtypes = [vp, i32_p, i32_p, d_p, C.c_double, i, d_p, i32_p, i]
     L.cs_cuboid_draw_edges.argtypes = [vp, i32_p]
     L.cs_debug_edlines.argtypes = [vp, i, u8_p, C.POINTER(C.c_int16), C.POINTER(C.c_int16), C.POINTER(C.c_int16), u8_p, i32_p, i32_p, u8_p, f_p, i32_p, i]
     L.cs_comm_unique_id.argtypes = [vp, C.c_char_p, u8_p]
@@ -247,7 +253,7 @@ def load():
         L.cs_detect_descrip_lines_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), vp, u8_p, C.c_int32, i32_p]
         L.cs_lbd_compute_batch_device.argtypes = [vp, df_p, vp, i32_p, u8_p, f_p]
     for name in EXPORTS:
-        if name in DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS + LSD_DEBUG_EXPORTS + LBD_DEVICE_FRAME_EXPORTS and not hasattr(L, name):
+        if name in DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS + LSD_DEBUG_EXPORTS + NFA_DEBUG_EXPORTS + LBD_DEVICE_FRAME_EXPORTS and not hasattr(L, name):
             continue
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("cs_abi_version",):

@@ -60,12 +60,16 @@ __device__ __forceinline__ bool cs_nfa_double_equal(double a, double b)
     return (abs_diff / abs_max) <= (100.0 * DBL_EPSILON);
 }
 
-/* all 32 lanes call with the same arguments; lsd_first_term selects lsd.cpp's (n + 1) in place of log_gamma(n + 1) */
-static __device__ __noinline__ double cs_nfa_warp(const double *__restrict__ lgamma_table, int n, int k, double p, double logNT, bool lsd_first_term)
+/* all 32 lanes call with the same arguments; lsd_first_term selects lsd.cpp's (n + 1) in place of log_gamma(n + 1).  kBreak (cs_debug_nfa
+ * only) also reports the i at which the tail loop stopped: n + 1 when it ran to the end, -1 for the early returns and the underflow branch. */
+template <bool kBreak>
+__device__ __forceinline__ double cs_nfa_warp_impl(const double *__restrict__ lgamma_table, int n, int k, double p, double logNT, bool lsd_first_term,
+                                                   int *i_break)
 {
     const unsigned FULL = 0xffffffffu;
     const int lane = threadIdx.x & 31;
     const double LN10 = 2.30258509299404568402, tolerance = 0.1;
+    if (kBreak) *i_break = -1;
     if (n == 0 || k == 0) return -logNT;
     if (n == k) return -logNT - (double)n * log10(p);
     const double p_term = p / (1.0 - p);
@@ -77,6 +81,7 @@ static __device__ __noinline__ double cs_nfa_warp(const double *__restrict__ lga
         return -logNT;
     }
     double bin_tail = term;
+    if (kBreak) *i_break = n + 1;
     for (int i0 = k + 1; i0 <= n; i0 += 32) {
         const int i = i0 + lane;
         const bool valid = i <= n;
@@ -104,9 +109,18 @@ static __device__ __noinline__ double cs_nfa_warp(const double *__restrict__ lga
         const int src = hit ? (__ffs(hit) - 1) : (n_valid - 1);
         term = __shfl_sync(FULL, my_term, src);
         bin_tail = __shfl_sync(FULL, my_tail, src);
-        if (hit) break;
+        if (hit) {
+            if (kBreak) *i_break = i0 + src;
+            break;
+        }
     }
     return -log10(bin_tail) - logNT;
+}
+
+/* what the detectors call */
+static __device__ __noinline__ double cs_nfa_warp(const double *__restrict__ lgamma_table, int n, int k, double p, double logNT, bool lsd_first_term)
+{
+    return cs_nfa_warp_impl<false>(lgamma_table, n, k, p, logNT, lsd_first_term, nullptr);
 }
 #endif /* __CUDACC__ */
 

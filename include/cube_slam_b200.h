@@ -442,6 +442,13 @@ int cs_cuboid_draw_edges(const cs_cuboid_rec *rec, int32_t edges[12][8]);
 int cs_debug_atan2(cs_ctx *ctx, const double *y, const double *x, double *out, int n);
 double cs_atan2_host(double y, double x);
 
+/* The number-of-false-alarms test both line detectors end with (cube_slam_b200/csrc/cs_nfa.cuh: lsd.cpp's nfa with lsd_first_term = 1,
+ * descriptor.hpp's with 0), evaluated on the device by one warp per (n[i], k[i], p[i]) with the log_gamma table the detectors use (tests):
+ * out_value[i] the NFA, out_break[i] the i at which the binomial tail's loop stopped (n + 1: it ran to the end; -1: an early return or the
+ * underflow branch). */
+int cs_debug_nfa(cs_ctx *ctx, const int32_t *n, const int32_t *k, const double *p, double logNT, int lsd_first_term, double *out_value,
+                 int32_t *out_break, int count);
+
 /* ---- multi-GPU -------------------------------------------------------------------------- */
 /* Frames shard across ranks; the only exchange is one all-gather of the top-K record buffers.
  * No reference counterpart (the reference is single process); see BASELINE.json north_star. */

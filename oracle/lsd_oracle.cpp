@@ -185,6 +185,62 @@ inline double log_gamma_lanczos(double x)
 }
 inline double log_gamma(double x) { return x > 15.0 ? log_gamma_windschitl(x) : log_gamma_lanczos(x); }
 
+/* Optional statistics of one lsd_orc_detect call (lsd_orc_detect_stats), in the terms of the GPU seed loop (cs_lsd.cu: k_lsd_grow_seq keeps
+ * the first LSD_SEQ_SCAP = 2 048 entries of a seed's region list in shared memory, the rest in HBM; the refine re-grow is written behind the
+ * first pass, at base = first-pass size, so a seed's list holds n_all = first pass + re-grow entries, or the first pass alone when refine
+ * did not re-grow).  Collecting them changes no result. */
+enum {
+    ST_SEEDS = 0,          /* seeds grown (region_grow from the raster scan) */
+    ST_FIRST_SUM,          /* sum of first-pass region sizes */
+    ST_NALL_SPILL,         /* seeds with n_all > 2 048 */
+    ST_REGROW_PAST,        /* refine re-grows that start at list position >= 2 048 */
+    ST_REDUCE_PAST,        /* reduce_region_radius iterations on a list (base + region) longer than 2 048 */
+    ST_FIRST_MAX,          /* largest first pass */
+    ST_NALL_MAX,           /* largest n_all */
+    ST_FIRST_2047,         /* first passes of exactly 2 047, 2 048, 2 049 entries (three slots) */
+    ST_NALL_2047 = ST_FIRST_2047 + 3, /* n_all of exactly 2 047, 2 048, 2 049 (three slots) */
+    ST_NFA_MAX_N = ST_NALL_2047 + 3,  /* largest n of an nfa() call */
+    ST_NFA_PAST_TABLE,     /* nfa() calls that evaluate log_gamma(k + 1) or log_gamma(n - k + 1) at an argument >= 16 384 */
+    ST_COUNT
+};
+const int kSpill = 2048;         /* cs_lsd.cu LSD_SEQ_SCAP */
+const int kLgammaTable = 16384;  /* cs_nfa.cuh CS_LGAMMA_TABLE */
+thread_local int64_t *t_stats = nullptr;
+
+/* lsd.cpp:1100-1136 (lsd_first_term) or descriptor.hpp:763-830 (log_gamma(n + 1) as the first term).  i_break: the i at which the tail
+ * loop broke, n + 1 when it ran to the end, -1 for the early returns and the underflow branch. */
+double nfa_tail(int n, int k, double p, double logNT, bool lsd_first_term, int *i_break)
+{
+    if (i_break) *i_break = -1;
+    if (t_stats && n > t_stats[ST_NFA_MAX_N]) t_stats[ST_NFA_MAX_N] = n;
+    if (n == 0 || k == 0) return -logNT;
+    if (n == k) return -logNT - double(n) * std::log10(p);
+    if (t_stats && (k + 1 >= kLgammaTable || n - k + 1 >= kLgammaTable)) t_stats[ST_NFA_PAST_TABLE]++;
+    const double p_term = p / (1 - p);
+    const double first = lsd_first_term ? (double(n) + 1) : log_gamma(double(n) + 1.0);
+    const double log1term = first - log_gamma(double(k) + 1) - log_gamma(double(n - k) + 1) + double(k) * std::log(p) + double(n - k) * std::log(1.0 - p);
+    double term = std::exp(log1term);
+    if (double_equal(term, 0)) {
+        if (k > n * p) return -log1term / kLN10 - logNT;
+        return -logNT;
+    }
+    double bin_tail = term;
+    const double tolerance = 0.1;
+    int i = k + 1;
+    for (; i <= n; ++i) {
+        const double bin_term = double(n - i + 1) / double(i);
+        const double mult_term = bin_term * p_term;
+        term *= mult_term;
+        bin_tail += term;
+        if (bin_term < 1) {
+            const double err = term * ((1 - std::pow(mult_term, double(n - i + 1))) / (1 - mult_term) - 1);
+            if (err < tolerance * std::fabs(-std::log10(bin_tail) - logNT) * bin_tail) break;
+        }
+    }
+    if (i_break) *i_break = i;
+    return -std::log10(bin_tail) - logNT;
+}
+
 struct Rect {
     double x1, y1, x2, y2, width, x, y, theta, dx, dy, prec, p;
 };
@@ -196,6 +252,7 @@ struct Lsd {
     std::vector<int> list;  /* pixel addresses in pseudo-order (descending gradient bins) */
     std::vector<int> reg;   /* region: pixel addresses (angle / modgrad are looked up, they never change) */
     double LOG_NT = 0;
+    int cur_base = 0, cur_n_all = 0; /* statistics: where the current seed's re-grow starts in the GPU's region list, and the list's length */
 
     /* lsd.cpp:1138-1154 */
     bool is_aligned(int address, double theta, double prec) const
@@ -350,6 +407,7 @@ struct Lsd {
         const double radSq1 = dist_sq(xc, yc, rec.x1, rec.y1), radSq2 = dist_sq(xc, yc, rec.x2, rec.y2);
         double radSq = radSq1 > radSq2 ? radSq1 : radSq2;
         while (density < density_th) {
+            if (t_stats && cur_base + reg_size > kSpill) t_stats[ST_REDUCE_PAST]++;
             radSq *= 0.75 * 0.75;
             for (int i = 0; i < reg_size; ++i) {
                 if (dist_sq(xc, yc, double(reg[i] % W), double(reg[i] / W)) > radSq) {
@@ -386,7 +444,10 @@ struct Lsd {
         }
         const double mean_angle = sum / double(n);
         const double tau = 2.0 * std::sqrt((s_sum - 2.0 * mean_angle * sum) / double(n) + mean_angle * mean_angle);
+        cur_base = reg_size;
+        if (t_stats && cur_base >= kSpill) t_stats[ST_REGROW_PAST]++;
         region_grow(reg[0], reg_size, reg_angle, tau);
+        cur_n_all = cur_base + reg_size;
         if (reg_size < 2) return false;
         region2rect(reg_size, reg_angle, prec, p, rec);
         density = double(reg_size) / (dist2(rec.x1, rec.y1, rec.x2, rec.y2) * rec.width);
@@ -395,31 +456,7 @@ struct Lsd {
     }
 
     /* lsd.cpp:1100-1136 */
-    double nfa(int n, int k, double p) const
-    {
-        if (n == 0 || k == 0) return -LOG_NT;
-        if (n == k) return -LOG_NT - double(n) * std::log10(p);
-        const double p_term = p / (1 - p);
-        const double log1term = (double(n) + 1) - log_gamma(double(k) + 1) - log_gamma(double(n - k) + 1) + double(k) * std::log(p) + double(n - k) * std::log(1.0 - p);
-        double term = std::exp(log1term);
-        if (double_equal(term, 0)) {
-            if (k > n * p) return -log1term / kLN10 - LOG_NT;
-            return -LOG_NT;
-        }
-        double bin_tail = term;
-        const double tolerance = 0.1;
-        for (int i = k + 1; i <= n; ++i) {
-            const double bin_term = double(n - i + 1) / double(i);
-            const double mult_term = bin_term * p_term;
-            term *= mult_term;
-            bin_tail += term;
-            if (bin_term < 1) {
-                const double err = term * ((1 - std::pow(mult_term, double(n - i + 1))) / (1 - mult_term) - 1);
-                if (err < tolerance * std::fabs(-std::log10(bin_tail) - LOG_NT) * bin_tail) break;
-            }
-        }
-        return -std::log10(bin_tail) - LOG_NT;
-    }
+    double nfa(int n, int k, double p) const { return nfa_tail(n, k, p, LOG_NT, true, nullptr); }
 
     /* lsd.cpp:977-1098, including the vendored slips (tailp->p.x where y is meant; int/int slopes) */
     double rect_nfa(const Rect &rec) const
@@ -653,11 +690,32 @@ extern "C" int lsd_orc_detect(const uint8_t *img, int w, int h, int stride, int 
             int reg_size;
             double reg_angle;
             L.region_grow(adx, reg_size, reg_angle, prec);
-            if (reg_size < min_reg_size) continue;
+            L.cur_base = 0;
+            L.cur_n_all = reg_size;
+            if (t_stats) {
+                t_stats[ST_SEEDS]++;
+                t_stats[ST_FIRST_SUM] += reg_size;
+                t_stats[ST_FIRST_MAX] = std::max<int64_t>(t_stats[ST_FIRST_MAX], reg_size);
+                if (std::abs(reg_size - kSpill) <= 1) t_stats[ST_FIRST_2047 + reg_size - (kSpill - 1)]++;
+            }
+            /* the seed's list length once region_grow / refine are done with it */
+            auto note_n_all = [&L]() {
+                if (!t_stats) return;
+                const int n_all = L.cur_n_all;
+                if (n_all > kSpill) t_stats[ST_NALL_SPILL]++;
+                t_stats[ST_NALL_MAX] = std::max<int64_t>(t_stats[ST_NALL_MAX], n_all);
+                if (std::abs(n_all - kSpill) <= 1) t_stats[ST_NALL_2047 + n_all - (kSpill - 1)]++;
+            };
+            if (reg_size < min_reg_size) {
+                note_n_all();
+                continue;
+            }
             Rect rec;
             L.region2rect(reg_size, reg_angle, prec, p, rec);
+            const bool refined = refine_mode > 0 && L.refine(reg_size, reg_angle, prec, p, rec, DENSITY_TH);
+            note_n_all();
             if (refine_mode > 0) {
-                if (!L.refine(reg_size, reg_angle, prec, p, rec, DENSITY_TH)) continue;
+                if (!refined) continue;
                 if (refine_mode >= 2) {
                     const double log_nfa = L.rect_improve(rec);
                     if (log_nfa <= LOG_EPS) continue;
@@ -710,4 +768,35 @@ extern "C" int lsd_orc_detect(const uint8_t *img, int w, int h, int stride, int 
         n_out++;
     }
     return n_out;
+}
+
+/* lsd_orc_detect with its statistics (stats: ST_COUNT = 15 int64, zeroed here; see the enum above) */
+extern "C" int lsd_orc_detect_stats(const uint8_t *img, int w, int h, int stride, int channels, float line_length_thres, float *lines_out, int cap,
+                                    float *raw_lines, int cap_raw, int *n_raw_out, int refine_mode, int64_t *stats)
+{
+    static_assert(ST_COUNT == 15, "pyoracle.LSD_STAT_NAMES names 15 slots");
+    std::memset(stats, 0, sizeof(int64_t) * ST_COUNT);
+    t_stats = stats;
+    const int n = lsd_orc_detect(img, w, h, stride, channels, line_length_thres, lines_out, cap, raw_lines, cap_raw, n_raw_out, nullptr, nullptr,
+                                 nullptr, nullptr, nullptr, refine_mode);
+    t_stats = nullptr;
+    return n;
+}
+
+/* the reference's nfa on its own: lsd.cpp's ((n + 1) first term, lsd_first_term = 1) or descriptor.hpp's (log_gamma(n + 1)); i_break: the i at
+ * which the tail loop stopped (n + 1: it ran to the end), -1 for the early returns and the underflow branch */
+extern "C" double orc_lsd_nfa(int n, int k, double p, double logNT, int lsd_first_term, int *i_break)
+{
+    return nfa_tail(n, k, p, logNT, lsd_first_term != 0, i_break);
+}
+
+/* the same over arrays (one logNT and form for all) */
+extern "C" void orc_lsd_nfa_many(const int32_t *n, const int32_t *k, const double *p, int count, double logNT, int lsd_first_term, double *out,
+                                 int32_t *i_break)
+{
+    for (int i = 0; i < count; i++) {
+        int b = -1;
+        out[i] = nfa_tail(n[i], k[i], p[i], logNT, lsd_first_term != 0, &b);
+        i_break[i] = b;
+    }
 }

@@ -278,6 +278,53 @@ def lsd_detect(img, line_length_thres=15.0, cap=8192, want_stages=False, refine_
     return res
 
 
+LSD_STAT_NAMES = ("seeds", "first_sum", "n_all_spill", "regrow_past", "reduce_past", "first_max", "n_all_max",
+                  "first_2047", "first_2048", "first_2049", "n_all_2047", "n_all_2048", "n_all_2049", "nfa_max_n", "nfa_past_table")
+
+
+def lsd_stats(img, cap=16384):
+    """lsd_detect's raw segments and what the call did, in the GPU seed loop's terms (oracle/lsd_oracle.cpp, lsd_orc_detect_stats): seeds grown,
+    the sum of first-pass region sizes, seeds whose region list (n_all = first pass + refine's re-grow) is longer than the 2 048 entries the
+    seed loop keeps in shared memory, re-grows that start at or past entry 2 048, reduce-radius iterations on a list longer than 2 048, the
+    largest first pass and n_all, how many first passes / n_all were exactly 2 047, 2 048, 2 049, the largest NFA n and the NFA calls that take
+    log_gamma at an argument past the device's 16 384-entry table.  -> (raw n x 4 float32, dict)"""
+    img = np.ascontiguousarray(img, np.uint8)
+    h, w = img.shape[:2]
+    ch = 1 if img.ndim == 2 else img.shape[2]
+    out = np.zeros((cap, 4), np.float32)
+    raw = np.zeros((cap, 4), np.float32)
+    n_raw = C.c_int(0)
+    st = np.zeros(len(LSD_STAT_NAMES), np.int64)
+    L = lib()
+    L.lsd_orc_detect_stats.restype = C.c_int
+    L.lsd_orc_detect_stats(_p(img, C.c_uint8), w, h, img.strides[0], ch, C.c_float(15.0), _p(out, C.c_float), cap, _p(raw, C.c_float), cap,
+                           C.byref(n_raw), 2, _p(st, C.c_int64))
+    return raw[:min(n_raw.value, cap)].copy(), {k: int(v) for k, v in zip(LSD_STAT_NAMES, st)}
+
+
+def lsd_nfa(n, k, p, logNT, lsd_first_term=True):
+    """The reference's nfa(n, k, p) (lsd.cpp's (n + 1) first term, or descriptor.hpp's log_gamma(n + 1)) -> (value, i at which the tail loop
+    stopped: n + 1 when it ran to the end, -1 for the early returns and the underflow branch)"""
+    L = lib()
+    L.orc_lsd_nfa.restype = C.c_double
+    L.orc_lsd_nfa.argtypes = [C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.POINTER(C.c_int)]
+    b = C.c_int(0)
+    v = L.orc_lsd_nfa(int(n), int(k), float(p), float(logNT), int(bool(lsd_first_term)), C.byref(b))
+    return v, b.value
+
+
+def lsd_nfa_many(n, k, p, logNT, lsd_first_term=True):
+    """lsd_nfa over arrays (one logNT and form for all) -> (values float64, break indices int32)"""
+    n = np.ascontiguousarray(n, np.int32)
+    k = np.ascontiguousarray(k, np.int32)
+    p = np.ascontiguousarray(np.broadcast_to(p, n.shape), np.float64)
+    out = np.zeros(len(n))
+    brk = np.zeros(len(n), np.int32)
+    lib().orc_lsd_nfa_many(_p(n, C.c_int32), _p(k, C.c_int32), _p(p, C.c_double), len(n), C.c_double(logNT), int(bool(lsd_first_term)),
+                           _p(out, C.c_double), _p(brk, C.c_int32))
+    return out, brk
+
+
 _REF_LSD = None
 _REF_LSD_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref", "liblsd_ref.so")
 

@@ -214,15 +214,27 @@ def test_sequence_against_the_shipped_matlab_cuboids(det, fixture_b):
 
 
 def test_seed_loop_on_a_giant_region(det, oracle):
-    """A smooth ramp is one line-support region far larger than the shared-memory part of the region list (it spills to HBM):
-    result unchanged."""
-    ramp = np.tile((np.arange(640) * 0.35).astype(np.uint8)[None, :], (480, 1))
-    ramp = np.ascontiguousarray(ramp)
-    got = det.detect_filter_lines_batch(ramp[None])
-    _, redo = det.seed_loop_stats(1)
-    ref = oracle.lsd_detect(ramp, 15.0)
+    """A sawtooth ramp (8 gray levels per pixel, wrapping every 32 pixels) is a set of line-support regions of up to 8 809 pixels, far more
+    than the 2 048 entries of the region list the seed loop keeps in shared memory: the rest spill to HBM.  The profiling instantiation
+    counts those seeds (slot 8 of cs_debug_lsd_prof) exactly as the oracle does; the result is the oracle's."""
+    import ctypes as C
+    from test_oracle_ref_lsd_large_regions import sawtooth
+    saw = sawtooth(640, 480, 0, 8)
+    ctx = det._ctx
+    ctx.set_profiling(1)
+    try:
+        ctx.check(ctx.L.cs_debug_lsd_prof(ctx.h, None, 1))
+        got = det.detect_filter_lines_batch(saw[None])
+        prof = np.zeros(16, np.uint64)
+        ctx.check(ctx.L.cs_debug_lsd_prof(ctx.h, prof.ctypes.data_as(C.POINTER(C.c_uint64)), 0))
+    finally:
+        ctx.set_profiling(0)
+    raw, st = oracle.lsd_stats(saw)
+    assert int(prof[8]) == st["n_all_spill"] > 0
+    ref = oracle.lsd_detect(saw, 15.0)
     np.testing.assert_array_equal(got[0], ref["lines"])
     np.testing.assert_array_equal(det.debug_frame(0)["raw_lines"], ref["raw_lines"])
+    np.testing.assert_array_equal(raw, ref["raw_lines"])
 
 
 def test_tma_staged_tiles_equal_byte_staged_tiles(det, oracle):
