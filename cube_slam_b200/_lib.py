@@ -58,6 +58,9 @@ CUBOID_DTYPE = np.dtype([
 KEYLINE_DTYPE = np.dtype([("start_x", "f4"), ("start_y", "f4"), ("end_x", "f4"), ("end_y", "f4"), ("angle", "f4"), ("line_length", "f4"),
                           ("response", "f4"), ("size", "f4"), ("num_pixels", "i4"), ("class_id", "i4")])
 DMATCH_DTYPE = np.dtype([("query_idx", "i4"), ("train_idx", "i4"), ("img_idx", "i4"), ("distance", "f4")])
+# numpy view of cs_keyline_octave (64 bytes): KEYLINE_DTYPE's fields, then the in-octave end points and the octave
+OCTAVE_KEYLINE_DTYPE = np.dtype(KEYLINE_DTYPE.descr + [("s_oct_x", "f4"), ("s_oct_y", "f4"), ("e_oct_x", "f4"), ("e_oct_y", "f4"), ("octave", "i4"),
+                                                        ("pad_", "i4")])
 
 class DeviceFrames(C.Structure):
     """cs_device_frames: n_frames x height x width x channels bytes in device memory, byte strides."""
@@ -151,6 +154,11 @@ EXPORTS += NFA_DEBUG_EXPORTS
 # CPU test suite compiles do not have them
 LBD_DEVICE_FRAME_EXPORTS = ["cs_detect_descrip_lines_batch_device", "cs_lbd_compute_batch_device"]
 EXPORTS += LBD_DEVICE_FRAME_EXPORTS
+# every octave of a multi-octave LSD detector (cs_lbd_octaves.cu, cs_ingest.cu), bound the same way: the host builds of cs_lbd.cu and
+# cs_context.cu that the CPU test suite compiles do not have them
+OCTAVE_EXPORTS = ["cs_detect_raw_lines_octaves_batch", "cs_detect_descrip_lines_octaves_batch", "cs_detect_raw_lines_octaves_batch_device",
+                  "cs_detect_descrip_lines_octaves_batch_device"]
+EXPORTS += OCTAVE_EXPORTS
 
 
 def load():
@@ -252,8 +260,15 @@ def load():
         df_p = C.POINTER(DeviceFrames)
         L.cs_detect_descrip_lines_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), vp, u8_p, C.c_int32, i32_p]
         L.cs_lbd_compute_batch_device.argtypes = [vp, df_p, vp, i32_p, u8_p, f_p]
+    if all(hasattr(L, n) for n in OCTAVE_EXPORTS):
+        df_p = C.POINTER(DeviceFrames)
+        L.cs_detect_raw_lines_octaves_batch.argtypes = [vp, vp, i, i, i, i, i, C.POINTER(LineParams), vp, C.c_int32, i32_p]
+        L.cs_detect_descrip_lines_octaves_batch.argtypes = [vp, vp, i, i, i, i, i, C.POINTER(LineParams), vp, u8_p, C.c_int32, i32_p]
+        L.cs_detect_raw_lines_octaves_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), vp, C.c_int32, i32_p]
+        L.cs_detect_descrip_lines_octaves_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), vp, u8_p, C.c_int32, i32_p]
     for name in EXPORTS:
-        if name in DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS + LSD_DEBUG_EXPORTS + NFA_DEBUG_EXPORTS + LBD_DEVICE_FRAME_EXPORTS and not hasattr(L, name):
+        if name in (DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS + LSD_DEBUG_EXPORTS + NFA_DEBUG_EXPORTS + LBD_DEVICE_FRAME_EXPORTS
+                    + OCTAVE_EXPORTS) and not hasattr(L, name):
             continue
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("cs_abi_version",):

@@ -299,4 +299,32 @@ int cs_lbd_compute_batch_device(cs_ctx *c, const cs_device_frames *frames, const
     return cs_lbd_compute_run(c, buf, true, F, W, H, W * ch, ch, keylines, keyline_offsets, desc32, desc72);
 }
 
+/* the octave calls on device frames: the frames go to the EDLines buffer (the LSD buffer takes the gray pyramid), then the host forms' body */
+static int octaves_device(cs_ctx *c, const cs_device_frames *frames, const cs_line_params *params, bool describe, cs_keyline_octave *keylines,
+                          uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    int rc;
+    if ((rc = check_on_ctx(c, frames))) return rc;
+    if ((rc = cs_lsd_octaves_check(c, frames->width, frames->height, params, keylines, desc32, describe, max_lines_per_octave, n_lines))) return rc;
+    cudaSetDevice(cs_ctx_device(c));
+    const int F = frames->n_frames, W = frames->width, H = frames->height, ch = frames->channels;
+    uint8_t *buf = cs_edl_frame_buffer(c, (size_t)F * H * W * ch);
+    if (!buf) return CS_ERR_CUDA;
+    if ((rc = ingest(c, frames, buf))) return rc;
+    return cs_lsd_octaves_run(c, buf, F, W, H, W * ch, ch, params, describe, keylines, desc32, max_lines_per_octave, n_lines);
+}
+
+int cs_detect_raw_lines_octaves_batch_device(cs_ctx *c, const cs_device_frames *frames, const cs_line_params *params, cs_keyline_octave *keylines,
+                                             int32_t max_lines_per_octave, int32_t *n_lines)
+{
+    return octaves_device(c, frames, params, false, keylines, nullptr, max_lines_per_octave, n_lines);
+}
+
+int cs_detect_descrip_lines_octaves_batch_device(cs_ctx *c, const cs_device_frames *frames, const cs_line_params *params, cs_keyline_octave *keylines,
+                                                 uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines)
+{
+    return octaves_device(c, frames, params, true, keylines, desc32, max_lines_per_octave, n_lines);
+}
+
 } /* extern "C" */

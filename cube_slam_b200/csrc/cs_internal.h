@@ -156,4 +156,21 @@ int cs_lbd_check_given(cs_ctx *c, int n_frames, const cs_keyline *keylines, cons
 int cs_lbd_compute_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int width, int height, int stride, int channels,
                        const cs_keyline *keylines, const int32_t *keyline_offsets, uint8_t *desc32, float *desc72);
 
+/* ---- every octave of a multi-octave LSD detector (cs_lbd_octaves.cu) */
+/* the raw segments of the last LSD run (accepted candidates in seed order, before the key-line filter): max_lines_per_frame x 4 floats per
+ * frame, and per frame their count (> the capacity when they did not fit) -- in HBM, until the next run (cs_lsd.cu) */
+void cs_lsd_raw_segments(cs_ctx *c, const float **d_raw, const int32_t **d_nraw);
+/* LSDDetector::detect's KeyLine fill (LSDDetector.cpp:205-250) for one LSD segment `raw` of octave `octave` (an ow x oh image, 2^octave =
+ * `scale`) of a w x h input frame: false when the border test drops it (cs_lbd.cu) */
+bool cs_keyline_from_lsd_octave(const float *raw, float scale, int ow, int oh, int w, int h, int octave, int class_id, cs_keyline_octave &o);
+/* the 32-byte descriptors of n key lines, line i of frame frame[i] of the n_frames x h x w Sobel maps d_dx / d_dy, to the host (cs_lbd.cu) */
+int cs_lbd_describe_keylines(cs_ctx *c, const cs_keyline *keylines, const int32_t *frame, int n, const int16_t *d_dx, const int16_t *d_dy, int w,
+                             int h, uint8_t *desc32);
+/* the body of the octave calls after their argument checks, on packed frames (rows of `stride` bytes) already on the device */
+int cs_lsd_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width, int height, int stride, int channels, const cs_line_params *params,
+                       bool describe, cs_keyline_octave *keylines, uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines);
+/* the octave calls' checks of params and max_lines_per_octave (the frames are checked by the caller) */
+int cs_lsd_octaves_check(cs_ctx *c, int width, int height, const cs_line_params *params, const void *keylines, const void *desc32, bool describe,
+                         int32_t max_lines_per_octave, const int32_t *n_lines);
+
 #endif

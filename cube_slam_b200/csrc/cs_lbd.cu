@@ -292,6 +292,50 @@ int cs_lbd_debug_prepare(const cs_keyline *keylines, int n, void *lines24, float
 
 }  // extern "C"
 
+/* ---- the octave calls (cs_lbd_octaves.cu) */
+bool cs_keyline_from_lsd_octave(const float *raw, float scale, int ow, int oh, int w, int h, int octave, int class_id, cs_keyline_octave &o)
+{
+    float e[4] = {raw[0], raw[1], raw[2], raw[3]}; /* checkLineExtremes against the octave's size (:75-101) */
+    if (e[0] < 0) e[0] = 0;
+    if (e[0] >= ow) e[0] = (float)ow - 1.0f;
+    if (e[2] < 0) e[2] = 0;
+    if (e[2] >= ow) e[2] = (float)ow - 1.0f;
+    if (e[1] < 0) e[1] = 0;
+    if (e[1] >= oh) e[1] = (float)oh - 1.0f;
+    if (e[3] < 0) e[3] = 0;
+    if (e[3] >= oh) e[3] = (float)oh - 1.0f;
+    const float sx = e[0] * scale, sy = e[1] * scale, ex = e[2] * scale, ey = e[3] * scale;
+    const float t = 10; /* pre_boundary_thre, against the input frame's size */
+    if (((sx < t) && (ex < t)) || ((sx > w - t) && (ex > w - t)) || ((sy < t) && (ey < t)) || ((sy > h - t) && (ey > h - t))) return false;
+    cs_keyline &kl = o.kl;
+    kl.start_x = sx;
+    kl.start_y = sy;
+    kl.end_x = ex;
+    kl.end_y = ey;
+    const double lx = (double)(e[0] - e[2]), ly = (double)(e[1] - e[3]); /* in-octave, as keyline_from_lsd_row */
+    kl.line_length = (float)sqrt(lx * lx + ly * ly);
+    kl.num_pixels = line_iterator_count(e[0], e[1], e[2], e[3], ow, oh); /* LineIterator on the octave image */
+    kl.angle = atan2f(ey - sy, ex - sx);
+    kl.size = (ex - sx) * (ey - sy);
+    kl.response = kl.line_length / std::max(ow, oh);
+    kl.class_id = class_id;
+    o.s_oct_x = e[0];
+    o.s_oct_y = e[1];
+    o.e_oct_x = e[2];
+    o.e_oct_y = e[3];
+    o.octave = octave;
+    o.pad_ = 0;
+    return true;
+}
+
+int cs_lbd_describe_keylines(cs_ctx *c, const cs_keyline *keylines, const int32_t *frame, int n, const int16_t *d_dx, const int16_t *d_dy, int w, int h,
+                             uint8_t *desc32)
+{
+    std::vector<CsLbdLine> lines((size_t)n);
+    for (int i = 0; i < n; i++) lbd_prepare(keylines[i], frame[i], lines[i]);
+    return describe(c, *state_of(c), lines, d_dx, d_dy, w, h, desc32, nullptr);
+}
+
 /* ---- shared by the host-frame entry points below and their device-frame forms (cs_ingest.cu) */
 int cs_lbd_check_given(cs_ctx *c, int n_frames, const cs_keyline *keylines, const int32_t *keyline_offsets, const uint8_t *desc32, int *n)
 {

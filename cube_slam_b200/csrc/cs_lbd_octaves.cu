@@ -1,0 +1,356 @@
+/* cs_lbd_octaves.cu -- every octave of a multi-octave LSD line_lbd_detect: the image pyramids, LSD per octave, the key lines and their LBD
+ * descriptors (include/cube_slam_b200.h: cs_detect_raw_lines_octaves_batch, cs_detect_descrip_lines_octaves_batch).
+ *
+ * Replaces   line_lbd/class/line_lbd_allclass.cpp:125-172,285-339   detect_raw_lines (both KeyLine overloads), detect_descrip_lines_octaves
+ *            line_lbd/libs/LSDDetector.cpp:55-72,176-250             computeGaussianPyramid, detect: LSD per octave, KeyLine fill
+ *            line_lbd/libs/binary_descriptor.cpp:352-398             computeGaussianPyramid + computeSobel for every octave
+ *
+ *   k_oct_gray      cvtColor of the frames (the fixed-point arithmetic of k_lsd_front / k_ed_front): octave 0 of the LSD pyramid
+ *   k_oct_pyrdown   cv::pyrDown on 8-bit planes: the separable 1-4-6-4-1 kernel at the even source positions, BORDER_REFLECT_101, one
+ *                   rounding (sum + 128) >> 8 (oracle/ref/minicv.hpp states it and pins it to cv2)
+ *   k_oct_blur5     GaussianBlur(5 x 5, sigma 1) of the gray plane: OpenCV's fixed-point kernel (14 62 104 62 14) in both directions, one
+ *                   rounding (sum + 32768) >> 16 -- what k_ed_front computes -- the base of the descriptor's pyramid
+ *   k_oct_sobel     3 x 3 Sobel to int16 (BORDER_REFLECT_101) of the descriptor's pyramid, octaves >= 1; octave 0's maps come from
+ *                   cs_edl_sobel_maps, as for the one-octave descriptor
+ * One thread per output pixel over the whole batch; every plane is a few hundred KB, bound by its bytes.  The LSD of each octave is the
+ * one-octave detector (cs_lsd_run_sync) on a gray plane; its raw segments go to the host, where the key lines are filled and filtered
+ * (cs_keyline_from_lsd_octave, cs_lbd.cu), and the descriptors are computed per octave by the one-octave descriptor kernel. */
+#include <cuda_runtime.h>
+#include <math.h>
+#include <stdint.h>
+#include <string.h>
+
+#include <algorithm>
+#include <cmath>
+#include <vector>
+
+#include "cs_internal.h"
+
+namespace {
+
+__device__ __forceinline__ int oct_reflect101(int p, int n)
+{
+    if (n == 1) return 0;
+    while (p < 0 || p >= n) p = (p < 0) ? -p : 2 * n - 2 - p;
+    return p;
+}
+
+__global__ void __launch_bounds__(256) k_oct_gray(const uint8_t *__restrict__ img, int n_frames, int w, int h, int stride, int channels,
+                                                  uint8_t *__restrict__ gray)
+{
+    const int64_t total = (int64_t)n_frames * w * h;
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < total; p += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t f = p / ((int64_t)w * h);
+        const int r = (int)(p - f * (int64_t)w * h);
+        const int y = r / w, x = r - y * w;
+        const uint8_t *row = img + ((size_t)f * h + y) * stride;
+        if (channels == 3) {
+            const uint8_t *q = row + 3 * x;
+            gray[p] = (uint8_t)((q[0] * 3735u + q[1] * 19235u + q[2] * 9798u + (1u << 14)) >> 15);
+        } else
+            gray[p] = row[x];
+    }
+}
+
+__global__ void __launch_bounds__(256) k_oct_pyrdown(const uint8_t *__restrict__ src, int n_frames, int sw, int sh, uint8_t *__restrict__ dst, int dw,
+                                                     int dh)
+{
+    const int64_t total = (int64_t)n_frames * dw * dh;
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < total; p += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t f = p / ((int64_t)dw * dh);
+        const int r = (int)(p - f * (int64_t)dw * dh);
+        const int y = r / dw, x = r - y * dw;
+        const uint8_t *s = src + (size_t)f * sw * sh;
+        const int k[5] = {1, 4, 6, 4, 1};
+        int xs[5];
+#pragma unroll
+        for (int i = 0; i < 5; i++) xs[i] = oct_reflect101(2 * x + i - 2, sw);
+        uint32_t a = 0;
+#pragma unroll
+        for (int j = 0; j < 5; j++) {
+            const uint8_t *row = s + (size_t)oct_reflect101(2 * y + j - 2, sh) * sw;
+            uint32_t t = 0;
+#pragma unroll
+            for (int i = 0; i < 5; i++) t += k[i] * (uint32_t)row[xs[i]];
+            a += k[j] * t;
+        }
+        dst[p] = (uint8_t)((a + 128u) >> 8);
+    }
+}
+
+__global__ void __launch_bounds__(256) k_oct_blur5(const uint8_t *__restrict__ src, int n_frames, int w, int h, uint8_t *__restrict__ dst)
+{
+    const int64_t total = (int64_t)n_frames * w * h;
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < total; p += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t f = p / ((int64_t)w * h);
+        const int r = (int)(p - f * (int64_t)w * h);
+        const int y = r / w, x = r - y * w;
+        const uint8_t *s = src + (size_t)f * w * h;
+        const int k[5] = {14, 62, 104, 62, 14};
+        int xs[5];
+#pragma unroll
+        for (int i = 0; i < 5; i++) xs[i] = oct_reflect101(x + i - 2, w);
+        uint32_t a = 0;
+#pragma unroll
+        for (int j = 0; j < 5; j++) {
+            const uint8_t *row = s + (size_t)oct_reflect101(y + j - 2, h) * w;
+            uint32_t t = 0;
+#pragma unroll
+            for (int i = 0; i < 5; i++) t += k[i] * (uint32_t)row[xs[i]];
+            a += k[j] * t;
+        }
+        dst[p] = (uint8_t)((a + 32768u) >> 16);
+    }
+}
+
+__global__ void __launch_bounds__(256) k_oct_sobel(const uint8_t *__restrict__ src, int n_frames, int w, int h, int16_t *__restrict__ dxo,
+                                                   int16_t *__restrict__ dyo)
+{
+    const int64_t total = (int64_t)n_frames * w * h;
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < total; p += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t f = p / ((int64_t)w * h);
+        const int r = (int)(p - f * (int64_t)w * h);
+        const int y = r / w, x = r - y * w;
+        const uint8_t *b = src + (size_t)f * w * h;
+        const int ym = oct_reflect101(y - 1, h), yp = oct_reflect101(y + 1, h), xm = oct_reflect101(x - 1, w), xp = oct_reflect101(x + 1, w);
+        const int a00 = b[(size_t)ym * w + xm], a01 = b[(size_t)ym * w + x], a02 = b[(size_t)ym * w + xp];
+        const int a10 = b[(size_t)y * w + xm], a12 = b[(size_t)y * w + xp];
+        const int a20 = b[(size_t)yp * w + xm], a21 = b[(size_t)yp * w + x], a22 = b[(size_t)yp * w + xp];
+        dxo[p] = (int16_t)((a02 + 2 * a12 + a22) - (a00 + 2 * a10 + a20));
+        dyo[p] = (int16_t)((a20 + 2 * a21 + a22) - (a00 + 2 * a01 + a02));
+    }
+}
+
+inline unsigned grid_for(int64_t n) { return (unsigned)std::min<int64_t>(std::max<int64_t>((n + 255) / 256, 1), CS_SM_COUNT * 32); }
+
+/* device scratch of one call, returned to the stream-ordered pool when the call ends */
+struct Scratch {
+    void *p = nullptr;
+    cudaStream_t st;
+    explicit Scratch(cudaStream_t s) : st(s) {}
+    ~Scratch()
+    {
+        if (p) cudaFreeAsync(p, st);
+    }
+};
+
+/* octave sizes: octave k is octave k - 1 halved with integer division (Size(cols / scale, rows / scale), scale 2) */
+void octave_sizes(int w, int h, int K, std::vector<int> &ow, std::vector<int> &oh)
+{
+    ow.assign((size_t)K, w);
+    oh.assign((size_t)K, h);
+    for (int k = 1; k < K; k++) {
+        ow[k] = ow[k - 1] / 2;
+        oh[k] = oh[k - 1] / 2;
+    }
+}
+
+}  // namespace
+
+int cs_lsd_octaves_check(cs_ctx *c, int width, int height, const cs_line_params *params, const void *keylines, const void *desc32, bool describe,
+                         int32_t max_lines_per_octave, const int32_t *n_lines)
+{
+    if (!params || !keylines || (describe && !desc32) || !n_lines || max_lines_per_octave <= 0)
+        return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
+    if (!params->use_LSD)
+        return cs_ctx_fail(c, CS_ERR_UNSUPPORTED, "the octave calls are provided for the LSD flavour (use_LSD = 1): EDLines groups its octaves differently");
+    const int K = params->numoctaves;
+    if (K < 1) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "numoctaves must be at least 1");
+    /* the reference passes the float ratio to an int scale (line_lbd_allclass.cpp:140); cv::pyrDown takes only |2 * dst - src| <= 2 */
+    if (K > 1 && !(params->octaveratio >= 2.0f && params->octaveratio < 3.0f))
+        return cs_ctx_fail(c, CS_ERR_INVALID_ARG,
+                           "numoctaves > 1 needs (int)octaveratio == 2 (got %g): cv::pyrDown makes an octave of (w / scale, h / scale) only when "
+                           "|2 * dst - src| <= 2",
+                           (double)params->octaveratio);
+    std::vector<int> ow, oh;
+    octave_sizes(width, height, K, ow, oh);
+    if (std::lrint(ow[K - 1] * 0.8) < 2 || std::lrint(oh[K - 1] * 0.8) < 2 || width > 32767 || height > 32767)
+        return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "octave %d of a %d x %d frame is %d x %d: too small for LSD", K - 1, width, height, ow[K - 1], oh[K - 1]);
+    return CS_OK;
+}
+
+int cs_lsd_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width, int height, int stride, int channels, const cs_line_params *params,
+                       bool describe, cs_keyline_octave *keylines, uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines)
+{
+    cudaSetDevice(cs_ctx_device(c));
+    cudaStream_t st = cs_ctx_stream(c);
+    const int F = n_frames, K = params->numoctaves, cap = max_lines_per_octave;
+    std::vector<int> ow, oh;
+    octave_sizes(width, height, K, ow, oh);
+    std::vector<size_t> off((size_t)K + 1, 0); /* plane k of every frame at off[k], frame f at off[k] + f * ow[k] * oh[k] */
+    for (int k = 0; k < K; k++) off[k + 1] = off[k] + (size_t)F * ow[k] * oh[k];
+
+    /* the LSD pyramid, in the LSD detector's frame buffer: LSD reads its octaves from there, and cs_debug_lsd of the last octave still can */
+    uint8_t *pyr = cs_lsd_frame_buffer(c, off[K]);
+    if (!pyr) return CS_ERR_CUDA;
+    k_oct_gray<<<grid_for((int64_t)off[1]), 256, 0, st>>>(d_imgs, F, width, height, stride, channels, pyr);
+    for (int k = 1; k < K; k++)
+        k_oct_pyrdown<<<grid_for((int64_t)(off[k + 1] - off[k])), 256, 0, st>>>(pyr + off[k - 1], F, ow[k - 1], oh[k - 1], pyr + off[k], ow[k], oh[k]);
+    cs_ctx_count_launches(c, K);
+    if (cudaGetLastError() != cudaSuccess) return cs_ctx_fail(c, CS_ERR_CUDA, "pyramid kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+
+    /* LSD per octave; the raw segments of each run to the host before the next run overwrites them, then the KeyLine fill */
+    std::vector<cs_keyline_octave> all((size_t)F * K * cap);
+    std::vector<int32_t> cnt((size_t)F * K, 0);
+    std::vector<float> raw((size_t)F * cap * 4);
+    std::vector<int32_t> nraw((size_t)F);
+    for (int k = 0; k < K; k++) {
+        const float *d_lines, *d_raw;
+        const int32_t *d_counts, *d_nraw;
+        const uint8_t *d_frames;
+        int rc;
+        if ((rc = cs_lsd_run_sync(c, pyr + off[k], true, F, ow[k], oh[k], ow[k], 1, params->line_length_thres, cap, &d_lines, &d_counts, &d_frames)))
+            return rc;
+        cs_lsd_raw_segments(c, &d_raw, &d_nraw);
+        if (cudaMemcpyAsync(nraw.data(), d_nraw, (size_t)F * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+            cudaMemcpyAsync(raw.data(), d_raw, raw.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+            return cs_ctx_fail(c, CS_ERR_CUDA, "LSD segment copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+        const float scale = (float)(1 << k);
+        for (int f = 0; f < F; f++) {
+            if (nraw[f] > cap)
+                return cs_ctx_fail(c, CS_ERR_CAPACITY, "frame %d, octave %d: %d LSD segments exceed max_lines_per_octave = %d", f, k, nraw[f], cap);
+            cs_keyline_octave *o = &all[((size_t)f * K + k) * cap];
+            int n = 0;
+            for (int i = 0; i < nraw[f]; i++)
+                if (cs_keyline_from_lsd_octave(&raw[((size_t)f * cap + i) * 4], scale, ow[k], oh[k], width, height, k, n, o[n])) n++;
+            cnt[(size_t)f * K + k] = n;
+        }
+    }
+    if (!describe) {
+        for (size_t s = 0; s < cnt.size(); s++) {
+            n_lines[s] = cnt[s];
+            if (cnt[s]) memcpy(keylines + s * cap, &all[s * cap], (size_t)cnt[s] * sizeof(cs_keyline_octave));
+        }
+        return CS_OK;
+    }
+
+    /* detect_descrip_lines_octaves' filter (:312-317): lineLength * (float)pow((float)octaveratio, octave) > line_length_thres */
+    size_t n_kept = 0;
+    std::vector<int32_t> kept_cnt(cnt.size(), 0);
+    for (int f = 0; f < F; f++)
+        for (int k = 0; k < K; k++) {
+            const float octave_scale = (float)std::pow(params->octaveratio, k);
+            const size_t s = (size_t)f * K + k;
+            cs_keyline_octave *o = &all[s * cap];
+            int n = 0;
+            for (int i = 0; i < cnt[s]; i++)
+                if (o[i].kl.line_length * octave_scale > params->line_length_thres) o[n++] = o[i];
+            kept_cnt[s] = n;
+            n_kept += n;
+        }
+    for (size_t s = 0; s < cnt.size(); s++) n_lines[s] = kept_cnt[s];
+    if (n_kept) {
+        /* the descriptor's pyramid: blurred octave 0, pyrDown per octave, Sobel of octaves >= 1 (octave 0's maps: cs_edl_sobel_maps) */
+        Scratch tmp(st);
+        const size_t hi = off[K] - off[1];
+        if (cudaMallocAsync(&tmp.p, off[K] + hi * 4 + 16, st) != cudaSuccess)
+            return cs_ctx_fail(c, CS_ERR_CUDA, "cudaMallocAsync(%zu) failed for the descriptor pyramid", off[K] + hi * 4 + 16);
+        uint8_t *blur = (uint8_t *)tmp.p;
+        int16_t *sob = (int16_t *)(((uintptr_t)(blur + off[K]) + 15) & ~(uintptr_t)15); /* dx of octave k at 2 * (off[k] - off[1]), dy after all dx */
+        k_oct_blur5<<<grid_for((int64_t)off[1]), 256, 0, st>>>(pyr, F, width, height, blur);
+        for (int k = 1; k < K; k++) {
+            k_oct_pyrdown<<<grid_for((int64_t)(off[k + 1] - off[k])), 256, 0, st>>>(blur + off[k - 1], F, ow[k - 1], oh[k - 1], blur + off[k], ow[k], oh[k]);
+            k_oct_sobel<<<grid_for((int64_t)(off[k + 1] - off[k])), 256, 0, st>>>(blur + off[k], F, ow[k], oh[k], sob + (off[k] - off[1]),
+                                                                                 sob + hi + (off[k] - off[1]));
+        }
+        cs_ctx_count_launches(c, 2 * K - 1);
+        if (cudaGetLastError() != cudaSuccess)
+            return cs_ctx_fail(c, CS_ERR_CUDA, "descriptor pyramid kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+        std::vector<cs_keyline> lines;
+        std::vector<int32_t> frame;
+        std::vector<uint8_t> packed;
+        for (int k = 0; k < K; k++) {
+            lines.clear();
+            frame.clear();
+            for (int f = 0; f < F; f++) {
+                const size_t s = (size_t)f * K + k;
+                for (int i = 0; i < kept_cnt[s]; i++) {
+                    const cs_keyline_octave &o = all[s * cap + i];
+                    cs_keyline kl = o.kl; /* computeLBD reads the in-octave ends, numOfPixels and angle (binary_descriptor.cpp:1207-1250) */
+                    kl.start_x = o.s_oct_x;
+                    kl.start_y = o.s_oct_y;
+                    kl.end_x = o.e_oct_x;
+                    kl.end_y = o.e_oct_y;
+                    lines.push_back(kl);
+                    frame.push_back(f);
+                }
+            }
+            if (lines.empty()) continue;
+            const int16_t *d_dx, *d_dy;
+            int rc;
+            if (k == 0) {
+                if ((rc = cs_edl_sobel_maps(c, pyr, true, F, width, height, width, 1, &d_dx, &d_dy))) return rc;
+            } else {
+                d_dx = sob + (off[k] - off[1]);
+                d_dy = sob + hi + (off[k] - off[1]);
+            }
+            packed.resize(lines.size() * 32);
+            if ((rc = cs_lbd_describe_keylines(c, lines.data(), frame.data(), (int)lines.size(), d_dx, d_dy, ow[k], oh[k], packed.data()))) return rc;
+            size_t row = 0;
+            for (int f = 0; f < F; f++) {
+                const size_t s = (size_t)f * K + k;
+                if (kept_cnt[s]) memcpy(desc32 + s * cap * 32, &packed[row * 32], (size_t)kept_cnt[s] * 32);
+                row += kept_cnt[s];
+            }
+        }
+    }
+    /* :319-330: start x <= end x (both pairs of ends swapped, the angle folded by normalize_to_PI in double), class_id within the octave */
+    const double PI = 3.14159265; /* line_lbd_allclass.cpp:19 */
+    for (size_t s = 0; s < cnt.size(); s++)
+        for (int i = 0; i < kept_cnt[s]; i++) {
+            cs_keyline_octave o = all[s * cap + i];
+            if (o.kl.start_x > o.kl.end_x) {
+                std::swap(o.kl.start_x, o.kl.end_x);
+                std::swap(o.kl.start_y, o.kl.end_y);
+                std::swap(o.s_oct_x, o.e_oct_x);
+                std::swap(o.s_oct_y, o.e_oct_y);
+                const float a = o.kl.angle;
+                if (a > PI / 2)
+                    o.kl.angle = (float)(a - PI);
+                else if (a < -PI / 2)
+                    o.kl.angle = (float)(a + PI);
+            }
+            o.kl.class_id = i;
+            keylines[s * cap + i] = o;
+        }
+    return CS_OK;
+}
+
+namespace {
+
+int octaves_host(cs_ctx *c, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels, const cs_line_params *params,
+                 bool describe, cs_keyline_octave *keylines, uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    if (!imgs || n_frames <= 0 || width <= 0 || height <= 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
+    if (channels != 1 && channels != 3) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "channels must be 1 or 3");
+    if (stride < width * channels) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "stride smaller than a row");
+    int rc;
+    if ((rc = cs_lsd_octaves_check(c, width, height, params, keylines, desc32, describe, max_lines_per_octave, n_lines))) return rc;
+    cudaSetDevice(cs_ctx_device(c));
+    const size_t bytes = (size_t)n_frames * height * stride;
+    uint8_t *buf = cs_edl_frame_buffer(c, bytes);
+    if (!buf) return CS_ERR_CUDA;
+    if (cudaMemcpyAsync(buf, imgs, bytes, cudaMemcpyHostToDevice, cs_ctx_stream(c)) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "H2D copy of frames failed");
+    return cs_lsd_octaves_run(c, buf, n_frames, width, height, stride, channels, params, describe, keylines, desc32, max_lines_per_octave, n_lines);
+}
+
+}  // namespace
+
+extern "C" {
+
+int cs_detect_raw_lines_octaves_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
+                                      const cs_line_params *params, cs_keyline_octave *keylines, int32_t max_lines_per_octave, int32_t *n_lines)
+{
+    return octaves_host(c, imgs, n_frames, width, height, stride, channels, params, false, keylines, nullptr, max_lines_per_octave, n_lines);
+}
+
+int cs_detect_descrip_lines_octaves_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
+                                          const cs_line_params *params, cs_keyline_octave *keylines, uint8_t *desc32, int32_t max_lines_per_octave,
+                                          int32_t *n_lines)
+{
+    return octaves_host(c, imgs, n_frames, width, height, stride, channels, params, true, keylines, desc32, max_lines_per_octave, n_lines);
+}
+
+}  // extern "C"

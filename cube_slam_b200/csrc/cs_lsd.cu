@@ -1552,6 +1552,13 @@ int cs_lsd_run_sync(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_f
     return CS_OK;
 }
 
+void cs_lsd_raw_segments(cs_ctx *c, const float **d_raw, const int32_t **d_nraw)
+{
+    LsdState *S = state_of(c);
+    *d_raw = (const float *)S->raw.p;
+    *d_nraw = (const int32_t *)S->nraw.p;
+}
+
 void cs_lsd_destroy(void *state)
 {
     LsdState *S = (LsdState *)state;

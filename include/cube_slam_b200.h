@@ -90,8 +90,10 @@ typedef struct cs_cuboid_rec {
  * line_lbd/libs/binary_descriptor.cpp:1511-1522). */
 typedef struct cs_line_params {
     int32_t use_LSD;            /* line_lbd_allclass.h:29; class default 0, object_slam sets 1 (main_obj.cpp:365) */
-    int32_t numoctaves;         /* :26, default 1.  Any value >= 1 gives the same result: only octave 0 survives filter_lines (:200-207) and
-                                   detect_descrip_lines (:239,266), and octave 0 does not depend on the higher ones */
+    int32_t numoctaves;         /* :26, default 1.  Any value >= 1 gives the same result in the octave-0 calls: only octave 0 survives
+                                   filter_lines (:200-207) and detect_descrip_lines (:239,266), and octave 0 does not depend on the higher
+                                   ones.  cs_detect_raw_lines_octaves_batch / cs_detect_descrip_lines_octaves_batch return every octave
+                                   (LSD flavour, (int)octaveratio == 2 when numoctaves > 1) */
     float octaveratio;          /* :27, default 1 */
     float line_length_thres;    /* :30, class default 50, object_slam uses 15 */
 } cs_line_params;
@@ -337,6 +339,44 @@ int cs_detect_descrip_lines(cs_ctx *ctx, const uint8_t *img, int width, int heig
 int cs_detect_descrip_lines_batch(cs_ctx *ctx, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
                                   const cs_line_params *params, cs_keyline *keylines, uint8_t *desc32, int32_t max_lines_per_frame,
                                   int32_t *n_lines /* n_frames */);
+
+/* Every octave of a multi-octave LSD detector (use_LSD = 1): the KeyLine of octave k with both pairs of end points.  kl.start / end are the
+ * points in the input frame (the in-octave points times 2^k), kl.response and kl.num_pixels are measured on the octave image, kl.class_id is
+ * the position in the octave's list.  KeyLine::pt is the mid point of kl's two ends. */
+typedef struct cs_keyline_octave {
+    cs_keyline kl;
+    float s_oct_x, s_oct_y, e_oct_x, e_oct_y; /* sPointInOctaveX / Y, ePointInOctaveX / Y */
+    int32_t octave;                           /* KeyLine::octave */
+    int32_t pad_;
+} cs_keyline_octave;
+
+/* line_lbd_detect::detect_raw_lines(gray, vector<KeyLine>&) and its vector<vector<KeyLine>> overload (line_lbd_allclass.cpp:125-172) for a
+ * detector built with numoctaves octaves, LSD flavour (LSDDetector.cpp:55-72,176-250): octave 0 is the gray frame, octave k is cv::pyrDown of
+ * octave k - 1 to (w / 2, h / 2); LSD runs on every octave; a segment's ends are clamped to its octave, scaled by 2^k and dropped when both
+ * lie within 10 px of the same border of the input frame.  Octave k of frame f is written at keylines + (f * numoctaves + k) *
+ * max_lines_per_octave, n_lines[f * numoctaves + k] of them (n_lines holds n_frames * numoctaves counts).  max_lines_per_octave bounds the
+ * segments LSD finds in one octave, before the border test.
+ * Errors: use_LSD == 0 is CS_ERR_UNSUPPORTED (EDLines groups its octaves differently); numoctaves < 1, or numoctaves > 1 with
+ * (int)octaveratio != 2 (pyrDown only halves an image: |2 * dst - src| <= 2), or a smallest octave too small for LSD is CS_ERR_INVALID_ARG;
+ * more segments than max_lines_per_octave in an octave is CS_ERR_CAPACITY, naming the frame and the octave.  Synchronous. */
+int cs_detect_raw_lines_octaves_batch(cs_ctx *ctx, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
+                                      const cs_line_params *params, cs_keyline_octave *keylines, int32_t max_lines_per_octave,
+                                      int32_t *n_lines /* n_frames * numoctaves */);
+/* line_lbd_detect::detect_descrip_lines_octaves(gray, keylines_out, line_descrips) (line_lbd_allclass.cpp:285-339) for the same detector:
+ * the key lines above whose lineLength * (float)pow(octaveratio, octave) > line_length_thres, with start x <= end x (both pairs of ends
+ * swapped and the angle folded into [-pi/2, pi/2] where needed), class_id the position in the octave's kept list, and their 32-byte LBD
+ * descriptors (binary_descriptor.cpp:603-790), read from the Sobel maps of the key line's octave at its in-octave ends before the swap.  The
+ * descriptor's pyramid is its own: GaussianBlur(5 x 5, sigma 1) of the gray frame, then pyrDown per octave, then Sobel 3 x 3.  Slots, counts,
+ * checks and errors as cs_detect_raw_lines_octaves_batch; desc32 slot (f, k) starts at row (f * numoctaves + k) * max_lines_per_octave. */
+int cs_detect_descrip_lines_octaves_batch(cs_ctx *ctx, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
+                                          const cs_line_params *params, cs_keyline_octave *keylines, uint8_t *desc32,
+                                          int32_t max_lines_per_octave, int32_t *n_lines /* n_frames * numoctaves */);
+/* the two calls above on frames already in GPU memory (cs_device_frames): the same outputs, checks and errors; the frames go to the EDLines
+ * detector's own buffer, as in cs_lbd_compute_batch_device.  Synchronous. */
+int cs_detect_raw_lines_octaves_batch_device(cs_ctx *ctx, const cs_device_frames *frames, const cs_line_params *params, cs_keyline_octave *keylines,
+                                             int32_t max_lines_per_octave, int32_t *n_lines);
+int cs_detect_descrip_lines_octaves_batch_device(cs_ctx *ctx, const cs_device_frames *frames, const cs_line_params *params,
+                                                 cs_keyline_octave *keylines, uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines);
 
 /* line_lbd_detect::match_line_descrip(query, train, good_matches, matching_dist_thres) (line_lbd_allclass.cpp:341-356) over
  * BinaryDescriptorMatcher::match (line_lbd/libs/binary_descriptor_matcher.cpp:196-262): for every query descriptor the train descriptor

@@ -153,3 +153,55 @@ extern "C" int shim_line_match(const uint8_t *q, int nq, const uint8_t *t, int n
         return -1;
     }
 }
+
+/* the shim's members for a detector with (numoctaves, octaveratio), LSD flavour: mode 0 detect_raw_lines(gray, vector<vector<KeyLine>>),
+ * 1 detect_raw_lines(gray, vector<KeyLine>) split by KeyLine::octave, 2 detect_descrip_lines_octaves.  kl_out: octave k's key lines at
+ * k * cap, 64 bytes each (cs_keyline_octave's layout: the 40 bytes above, the in-octave ends, the octave); desc_out likewise in 32-byte rows;
+ * counts[k] per octave.  Returns the number of octaves (-1: exception, -6: a KeyLine::pt that is not the mid point of its ends). */
+extern "C" int shim_lsd_octaves(const uint8_t *img, int w, int h, int channels, int numoctaves, float octaveratio, float line_length_thres, int mode,
+                                void *kl_out, uint8_t *desc_out, int32_t *counts, int cap)
+{
+    struct Rec {
+        float sx, sy, ex, ey, angle, len, response, size;
+        int32_t npx, class_id;
+        float osx, osy, oex, oey;
+        int32_t octave, pad_;
+    };
+    try {
+        line_lbd_detect det(numoctaves, octaveratio);
+        det.use_LSD = true;
+        det.line_length_thres = line_length_thres;
+        cv::Mat gray(h, w, channels == 3 ? CV_8UC3 : CV_8UC1);
+        std::memcpy(gray.data, img, (size_t)w * h * channels);
+        std::vector<std::vector<cv::line_descriptor::KeyLine>> kls;
+        std::vector<cv::Mat> descs;
+        if (mode == 0)
+            det.detect_raw_lines(gray, kls);
+        else if (mode == 1) {
+            std::vector<cv::line_descriptor::KeyLine> flat;
+            det.detect_raw_lines(gray, flat);
+            for (const auto &k : flat) {
+                if (k.octave >= (int)kls.size()) kls.resize(k.octave + 1);
+                kls[k.octave].push_back(k);
+            }
+        } else
+            det.detect_descrip_lines_octaves(gray, kls, descs);
+        for (size_t o = 0; o < kls.size(); o++) {
+            const int n = (int)kls[o].size();
+            if (n > cap) return -7;
+            counts[o] = n;
+            for (int i = 0; i < n; i++) {
+                const cv::line_descriptor::KeyLine &k = kls[o][i];
+                if (k.pt.x != (k.endPointX + k.startPointX) / 2 || k.pt.y != (k.endPointY + k.startPointY) / 2) return -6;
+                Rec &r = ((Rec *)kl_out)[o * (size_t)cap + i];
+                r = Rec{k.startPointX, k.startPointY, k.endPointX, k.endPointY, k.angle, k.lineLength, k.response, k.size, k.numOfPixels, k.class_id,
+                        k.sPointInOctaveX, k.sPointInOctaveY, k.ePointInOctaveX, k.ePointInOctaveY, k.octave, 0};
+                if (mode == 2) std::memcpy(desc_out + (o * (size_t)cap + i) * 32, descs[o].data + (size_t)i * 32, 32);
+            }
+        }
+        return (int)kls.size();
+    } catch (const std::exception &e) {
+        fprintf(stderr, "shim_lsd_octaves: %s\n", e.what());
+        return -1;
+    }
+}
