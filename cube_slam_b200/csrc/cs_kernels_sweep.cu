@@ -298,16 +298,12 @@ __device__ __forceinline__ bool rebuild_corners(const CsJob &jb, const CsFrame &
     return g_build_corners(jb, vps, g_top_x(jb, top_id), config_id, prm.shorted_edge_thre, c, vp1pos);
 }
 
-/* combined_score of an emitted record: the ranking key, except where the key stands in for a NaN score with +inf (NaN ranks last but is
- * still a cuboid).  There the record reports the reference's own sum, normalized_error + skew penalty of its skew_ratio
- * (box_proposal_detail.cpp:517-536), which is NaN when either term is. */
-__device__ __forceinline__ double g_record_score(double key, const cs_cuboid_rec &o, const cs_cuboid_params &prm)
-{
-    if (!isinf(key)) return key;
-    double skew_error = prm.weight_skew_error * g_max(o.skew_ratio - prm.nominal_skew_ratio, 0.0);
-    if (o.skew_ratio > prm.max_cut_skew) skew_error = 100;
-    return o.normalized_error + prm.weight_skew_error * skew_error;
-}
+/* w_score of a kept proposal that the 3D lift drops (a negative scale, box_proposal_detail.cpp:493): a NaN that no arithmetic produces
+ * (sign set, signalling), so that a NaN combined score -- still a cuboid, ranked after every number including +inf -- is never taken
+ * for it.  The final ranking orders the other scores by sort_key (NaN last) and then by position. */
+#define FU_DROPPED_BITS 0xfff0000000000001ull
+__device__ __forceinline__ double fu_dropped() { return __longlong_as_double((long long)FU_DROPPED_BITS); }
+__device__ __forceinline__ bool fu_is_dropped(double s) { return (uint64_t)__double_as_longlong(s) == FU_DROPPED_BITS; }
 
 extern __shared__ unsigned char fu_smem_raw[];
 
@@ -324,7 +320,7 @@ __global__ void __launch_bounds__(FU_THREADS) k_fuse_rank(const CsObj *__restric
     __shared__ int s_warp[FU_THREADS / 32];
     __shared__ int s_i[4];
     __shared__ double s_red[4][FU_THREADS / 32];
-    __shared__ double s_best_v[FU_THREADS / 32];
+    __shared__ uint64_t s_best_v[FU_THREADS / 32];
     __shared__ long long s_best_p[FU_THREADS / 32];
     __shared__ long long s_chosen[CS_MAX_TOPK];
     uint64_t *sm_key = reinterpret_cast<uint64_t *>(fu_smem_raw);
@@ -464,13 +460,12 @@ __global__ void __launch_bounds__(FU_THREADS) k_fuse_rank(const CsObj *__restric
             g_lift_to_3d(c, (double)config_id, (double)vp1pos, yaw, ps.ground, ps.T, fr.invK, o);
             double sc;
             if (o.scale[0] < 0 || o.scale[1] < 0 || o.scale[2] < 0)
-                sc = nan(""); /* dropped: scale should be positive (:493) */
+                sc = fu_dropped(); /* scale should be positive (:493) */
             else {
                 const double skew_ratio = g_max(o.scale[0], o.scale[1]) / g_min(o.scale[0], o.scale[1]);
                 double skew_error = prm.weight_skew_error * g_max(skew_ratio - prm.nominal_skew_ratio, 0.0);
                 if (skew_ratio > prm.max_cut_skew) skew_error = 100;
                 sc = comb + prm.weight_skew_error * skew_error;
-                if (isnan(sc)) sc = __longlong_as_double(0x7ff0000000000000ll); /* NaN ranks with +inf, still a cuboid */
             }
             score[i] = sc;
         }
@@ -481,11 +476,11 @@ __global__ void __launch_bounds__(FU_THREADS) k_fuse_rank(const CsObj *__restric
         __syncthreads();
     }
 
-    /* 4. final ranking over all height samples: K rounds of arg-min by (score, position) (:517-536) */
+    /* 4. final ranking over all height samples: K rounds of arg-min by (score key, position) (:517-536) */
     const int K = min(topk, CS_MAX_TOPK);
     int n_out = 0;
     for (int round = 0; round < K; round++) {
-        double bv = 0;
+        uint64_t bv = 0;
         long long bp = -1; /* position = (job index in object << 32) | kept index */
         for (int jj = 0; jj < ob.n_jobs; jj++) {
             const int job = ob.job_off + jj;
@@ -493,20 +488,21 @@ __global__ void __launch_bounds__(FU_THREADS) k_fuse_rank(const CsObj *__restric
             const int nk = job_counts[job * 2 + 1];
             for (int i = tid; i < nk; i += FU_THREADS) {
                 const double sc = w_score[co + i];
-                if (isnan(sc)) continue;
+                if (fu_is_dropped(sc)) continue;
+                const uint64_t k = sort_key(sc);
                 const long long p = ((long long)jj << 32) | (long long)i;
                 bool taken = false;
                 for (int r = 0; r < round; r++) taken |= (s_chosen[r] == p);
                 if (taken) continue;
-                if (bp < 0 || sc < bv || (sc == bv && p < bp)) {
-                    bv = sc;
+                if (bp < 0 || k < bv || (k == bv && p < bp)) {
+                    bv = k;
                     bp = p;
                 }
             }
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
-            const double ov = __shfl_xor_sync(0xffffffffu, bv, o);
+            const uint64_t ov = __shfl_xor_sync(0xffffffffu, bv, o);
             const long long op = __shfl_xor_sync(0xffffffffu, bp, o);
             if (op >= 0 && (bp < 0 || ov < bv || (ov == bv && op < bp))) {
                 bv = ov;
@@ -520,10 +516,10 @@ __global__ void __launch_bounds__(FU_THREADS) k_fuse_rank(const CsObj *__restric
         }
         __syncthreads();
         if (tid == 0) {
-            double v = 0;
+            uint64_t v = 0;
             long long p = -1;
             for (int k = 0; k < FU_THREADS / 32; k++) {
-                const double ov = s_best_v[k];
+                const uint64_t ov = s_best_v[k];
                 const long long op = s_best_p[k];
                 if (op >= 0 && (p < 0 || ov < v || (ov == v && op < p))) {
                     v = ov;
@@ -566,7 +562,7 @@ __global__ void __launch_bounds__(FU_THREADS) k_fuse_rank(const CsObj *__restric
                 o.camera_roll_delta = 0;
                 o.camera_pitch_delta = 0;
             }
-            o.combined_score = g_record_score(w_score[co + i], o, prm);
+            o.combined_score = w_score[co + i];
             o.proposal_index = raw;
             o.height_sample_id = jb.hs;
             o.valid = 1;
@@ -629,7 +625,10 @@ __device__ __forceinline__ double g_skew_of(const D2 *c, const CsPose &ps, const
     g_lift_scale(c, ps.ground, ps.T, invK, sc3);
     if (sc3[0] < 0 || sc3[1] < 0 || sc3[2] < 0) return nan("");
     const double r = g_max(sc3[0], sc3[1]) / g_min(sc3[0], sc3[1]);
-    return isnan(r) ? __longlong_as_double(0x7ff0000000000000ll) : r; /* NaN skew (degenerate lift) ranks as +inf, still a cuboid */
+    /* a NaN ratio (degenerate lift, both ground-plane scales 0) is returned as +inf so that k_fuse_warp does not read it as the NaN of a
+     * dropped proposal.  k_fuse_warp then cuts it to a finite score where k_fuse_rank and the oracle score it NaN; no known input reaches
+     * this (DESIGN.md section 2, "Every field of cs_cuboid_params off its default") */
+    return isnan(r) ? __longlong_as_double(0x7ff0000000000000ll) : r;
 }
 
 /* VP_support_edge_infos for ONE vanishing point by ONE lane (object_3d_util.cpp:380-425): a plain loop over the line set, so
@@ -970,12 +969,11 @@ __global__ void __launch_bounds__(32 * FW_WARPS) k_fuse_warp(const CsObj *__rest
             const double skew_ratio = c_skew[co + cand]; /* from the sweep; NaN == negative scale == dropped */
             double sc;
             if (isnan(skew_ratio))
-                sc = nan("");
+                sc = fu_dropped();
             else {
                 double skew_error = prm.weight_skew_error * g_max(skew_ratio - prm.nominal_skew_ratio, 0.0);
                 if (skew_ratio > prm.max_cut_skew) skew_error = 100;
                 sc = comb + prm.weight_skew_error * skew_error;
-                if (isnan(sc)) sc = __longlong_as_double(0x7ff0000000000000ll);
             }
             w_score[co + i] = sc;
             w_norm[co + i] = comb;
@@ -990,12 +988,12 @@ __global__ void __launch_bounds__(32 * FW_WARPS) k_fuse_warp(const CsObj *__rest
     }
     __threadfence_block();
     __syncwarp();
-    /* 4. final ranking: K rounds of arg-min by (score, position) */
+    /* 4. final ranking: K rounds of arg-min by (score key, position) */
     const int K = min(topk, CS_MAX_TOPK);
     long long chosen[CS_MAX_TOPK];
     int n_out = 0;
     for (int round = 0; round < K; round++) {
-        double bv = 0;
+        uint64_t bv = 0;
         long long bp = -1;
         for (int jj = 0; jj < ob.n_jobs; jj++) {
             const int job = ob.job_off + jj;
@@ -1003,20 +1001,21 @@ __global__ void __launch_bounds__(32 * FW_WARPS) k_fuse_warp(const CsObj *__rest
             const int nk = job_counts[job * 2 + 1];
             for (int i = lane; i < nk; i += 32) {
                 const double sc = w_score[co + i];
-                if (isnan(sc)) continue;
+                if (fu_is_dropped(sc)) continue;
+                const uint64_t k = sort_key(sc);
                 const long long p = ((long long)jj << 32) | (long long)i;
                 bool taken = false;
                 for (int r = 0; r < round; r++) taken |= (chosen[r] == p);
                 if (taken) continue;
-                if (bp < 0 || sc < bv || (sc == bv && p < bp)) {
-                    bv = sc;
+                if (bp < 0 || k < bv || (k == bv && p < bp)) {
+                    bv = k;
                     bp = p;
                 }
             }
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
-            const double ov = __shfl_xor_sync(FULL, bv, o);
+            const uint64_t ov = __shfl_xor_sync(FULL, bv, o);
             const long long op = __shfl_xor_sync(FULL, bp, o);
             if (op >= 0 && (bp < 0 || ov < bv || (ov == bv && op < bp))) {
                 bv = ov;
@@ -1056,7 +1055,7 @@ __global__ void __launch_bounds__(32 * FW_WARPS) k_fuse_warp(const CsObj *__rest
                 o.camera_roll_delta = 0;
                 o.camera_pitch_delta = 0;
             }
-            o.combined_score = g_record_score(w_score[co + i], o, prm);
+            o.combined_score = w_score[co + i];
             o.proposal_index = raw;
             o.height_sample_id = jb.hs;
             o.valid = 1;

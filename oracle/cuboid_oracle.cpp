@@ -740,6 +740,42 @@ extern "C" int orc_merge_break_lines(const double *lines, int n, double dist_thr
     return m;
 }
 
+/* the helpers detect_cuboid calls with its parameters, one call each (flat arrays as oracle/ref/cuboid_ref.cpp's ref_ entry points) */
+extern "C" void orc_vp_support_edge_infos(const double *vps, const double *mids, const double *angles, int n, double thre12_deg, double thre3_deg,
+                                          double *out)
+{
+    const P2 v[3] = {{vps[0], vps[1]}, {vps[2], vps[3]}, {vps[4], vps[5]}};
+    vp_support_edge_infos(v, mids, angles, n, thre12_deg, thre3_deg, out);
+}
+
+extern "C" double orc_box_edge_sum_dists(const float *dist, int dw, int dh, const double *corners16, const int *edges, int n_edges, int reweight)
+{
+    P2 c[8];
+    for (int i = 0; i < 8; i++) c[i] = {corners16[i], corners16[8 + i]};
+    return box_edge_sum_dists(dist, dw, dh, c, reinterpret_cast<const int(*)[2]>(edges), n_edges, reweight != 0);
+}
+
+extern "C" int orc_fuse_normalize_scores_v2(const double *dist_err, const double *angle_err, int n, double weight_vp_angle, int normalize,
+                                            double *combined, int *keep)
+{
+    std::vector<double> d(dist_err, dist_err + n), a(angle_err, angle_err + n), s;
+    std::vector<int> k;
+    fuse_normalize_scores_v2(d, a, s, k, weight_vp_angle, normalize != 0);
+    for (size_t i = 0; i < k.size(); i++) {
+        keep[i] = k[i];
+        combined[i] = s[i];
+    }
+    return (int)k.size();
+}
+
+extern "C" int orc_linespace_d(double start, double end, double step, double *out, int cap)
+{
+    std::vector<double> r;
+    linespace<double>(start, end, step, r);
+    for (int i = 0; i < (int)r.size() && i < cap; i++) out[i] = r[i];
+    return (int)r.size();
+}
+
 extern "C" void orc_default_params(orc_params *p)
 {
     p->consider_config_1 = 1;

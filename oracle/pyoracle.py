@@ -151,6 +151,64 @@ def merge_break_lines(lines, dist_thre=20.0, angle_thre_deg=5.0, len_thre=30.0):
     return out[:n].copy()
 
 
+def _vp_support(L, name, vps, mids, angles, thre12_deg, thre3_deg):
+    vps = np.ascontiguousarray(vps, np.float64).reshape(3, 2)
+    mids = np.ascontiguousarray(mids, np.float64).reshape(-1, 2)
+    angles = np.ascontiguousarray(angles, np.float64).reshape(-1)
+    out = np.zeros((3, 2))
+    getattr(L, name)(_p(vps, C.c_double), _p(mids, C.c_double), _p(angles, C.c_double), len(angles), C.c_double(thre12_deg),
+                     C.c_double(thre3_deg), _p(out, C.c_double))
+    return out
+
+
+def _box_edge_sum_dists(L, name, dist, corners, edges, reweight):
+    dist = np.ascontiguousarray(dist, np.float32)
+    corners = np.ascontiguousarray(corners, np.float64).reshape(2, 8)
+    edges = np.ascontiguousarray(edges, np.int32).reshape(-1, 2)
+    f = getattr(L, name)
+    f.restype = C.c_double
+    return f(_p(dist, C.c_float), dist.shape[1], dist.shape[0], _p(corners, C.c_double), _p(edges, C.c_int32), len(edges), int(bool(reweight)))
+
+
+def _fuse_normalize(L, name, dist_err, angle_err, weight_vp_angle, normalize):
+    d = np.ascontiguousarray(dist_err, np.float64)
+    a = np.ascontiguousarray(angle_err, np.float64)
+    comb = np.zeros(max(len(d), 1))
+    keep = np.zeros(max(len(d), 1), np.int32)
+    f = getattr(L, name)
+    f.restype = C.c_int
+    m = f(_p(d, C.c_double), _p(a, C.c_double), len(d), C.c_double(weight_vp_angle), int(bool(normalize)), _p(comb, C.c_double), _p(keep, C.c_int32))
+    return keep[:m].copy(), comb[:m].copy()
+
+
+def _linespace(L, name, start, end, step, cap=1024):
+    out = np.zeros(cap)
+    f = getattr(L, name)
+    f.restype = C.c_int
+    n = f(C.c_double(start), C.c_double(end), C.c_double(step), _p(out, C.c_double), cap)
+    return out[:min(n, cap)].copy()
+
+
+def vp_support_edge_infos(vps, mids, angles, thre12_deg=15.0, thre3_deg=10.0):
+    """VP_support_edge_infos (object_3d_util.cpp:380-425): 3 x 2 bounding edge angles per vanishing point, NaN where none supports it."""
+    return _vp_support(lib(), "orc_vp_support_edge_infos", vps, mids, angles, thre12_deg, thre3_deg)
+
+
+def box_edge_sum_dists(dist, corners, edges, reweight=True):
+    """box_edge_sum_dists (object_3d_util.cpp:427-453) on a float32 distance map; corners 2 x 8, edges n x 2 corner ids."""
+    return _box_edge_sum_dists(lib(), "orc_box_edge_sum_dists", dist, corners, edges, reweight)
+
+
+def fuse_normalize_scores_v2(dist_err, angle_err, weight_vp_angle=0.8, normalize=True):
+    """fuse_normalize_scores_v2 (object_3d_util.cpp:495-565) -> (kept indices, their combined scores)."""
+    return _fuse_normalize(lib(), "orc_fuse_normalize_scores_v2", dist_err, angle_err, weight_vp_angle, normalize)
+
+
+def linespace(start, end, step, cap=1024):
+    """linespace<double> (matrix_utils.cpp:350-363): the samples (the loop stops after 1001)."""
+    return _linespace(lib(), "orc_linespace_d", start, end, step, cap)
+
+
 def cam_pose(K, T):
     K = np.ascontiguousarray(K, np.float64)
     T = np.ascontiguousarray(T, np.float64)
@@ -417,15 +475,51 @@ def ref_detect_cuboid_available():
     return os.path.exists(_REF_CUB_PATH)
 
 
-def ref_detect_cuboid(img, K, T_wc, boxes, lines, params=None, cap_per_box=8):
-    """The reference's OWN detect_3d_cuboid::detect_cuboid (detect_3d_cuboid/src/*.cpp compiled from /root/reference into
-    oracle/_ref/libcuboid_ref.so against oracle/ref/minieigen.hpp / minicv.hpp, see oracle/ref/cuboid_ref.cpp), driven as
-    object_slam/src/main_obj.cpp:354-361,449 drives it.  Returns a list (one entry per box) of REF_CUBOID_DTYPE arrays, best first."""
+def _ref_cub():
     global _REF_CUB
     lib()
     if _REF_CUB is None:
         _REF_CUB = C.CDLL(_REF_CUB_PATH)
-        _REF_CUB.ref_detect_cuboid.restype = C.c_int
+        _REF_CUB.ref_detect_cuboid_skew.restype = C.c_int
+        _REF_CUB.ref_merge_break_lines.restype = C.c_int
+    return _REF_CUB
+
+
+def ref_merge_break_lines(lines, dist_thre=20.0, angle_thre_deg=5.0, len_thre=30.0):
+    """The reference's OWN merge_break_lines (object_3d_util.cpp:300)."""
+    lines = np.ascontiguousarray(lines, np.float64).reshape(-1, 4)
+    out = np.empty((max(len(lines), 1), 4))
+    n = _ref_cub().ref_merge_break_lines(_p(lines, C.c_double), len(lines), C.c_double(dist_thre), C.c_double(angle_thre_deg),
+                                         C.c_double(len_thre), _p(out, C.c_double))
+    return out[:n].copy()
+
+
+def ref_vp_support_edge_infos(vps, mids, angles, thre12_deg=15.0, thre3_deg=10.0):
+    """The reference's OWN VP_support_edge_infos (object_3d_util.cpp:380)."""
+    return _vp_support(_ref_cub(), "ref_vp_support_edge_infos", vps, mids, angles, thre12_deg, thre3_deg)
+
+
+def ref_box_edge_sum_dists(dist, corners, edges, reweight=True):
+    """The reference's OWN box_edge_sum_dists (object_3d_util.cpp:427)."""
+    return _box_edge_sum_dists(_ref_cub(), "ref_box_edge_sum_dists", dist, corners, edges, reweight)
+
+
+def ref_fuse_normalize_scores_v2(dist_err, angle_err, weight_vp_angle=0.8, normalize=True):
+    """The reference's OWN fuse_normalize_scores_v2 (object_3d_util.cpp:495)."""
+    return _fuse_normalize(_ref_cub(), "ref_fuse_normalize_scores_v2", dist_err, angle_err, weight_vp_angle, normalize)
+
+
+def ref_linespace(start, end, step, cap=1024):
+    """The reference's OWN linespace<double> (matrix_utils.cpp:350)."""
+    return _linespace(_ref_cub(), "ref_linespace_d", start, end, step, cap)
+
+
+def ref_detect_cuboid(img, K, T_wc, boxes, lines, params=None, cap_per_box=8):
+    """The reference's OWN detect_3d_cuboid::detect_cuboid (detect_3d_cuboid/src/*.cpp compiled from /root/reference into
+    oracle/_ref/libcuboid_ref.so against oracle/ref/minieigen.hpp / minicv.hpp, see oracle/ref/cuboid_ref.cpp), driven as
+    object_slam/src/main_obj.cpp:354-361,449 drives it, with the members of params it has (the configs, both sampling flags,
+    max_cuboid_num, nominal_skew_ratio, max_cut_skew).  Returns a list (one entry per box) of REF_CUBOID_DTYPE arrays, best first."""
+    _ref_cub()
     if params is None:
         params = default_params()
     img = np.ascontiguousarray(img, np.uint8)
@@ -439,9 +533,10 @@ def ref_detect_cuboid(img, K, T_wc, boxes, lines, params=None, cap_per_box=8):
     flags = np.array([params.consider_config_1, params.consider_config_2, params.whether_sample_cam_roll_pitch, params.whether_sample_bbox_height], np.int32)
     out = np.zeros((max(N, 1), cap_per_box), REF_CUBOID_DTYPE)
     counts = np.zeros(max(N, 1), np.int32)
-    rc = _REF_CUB.ref_detect_cuboid(_p(img, C.c_uint8), w, h, ch, _p(K, C.c_double), _p(T_wc, C.c_double), _p(boxes, C.c_double), N,
-                                    _p(lines, C.c_double), len(lines), _p(flags, C.c_int32), C.c_double(params.nominal_skew_ratio),
-                                    int(params.max_cuboid_num), out.ctypes.data_as(C.POINTER(C.c_double)), cap_per_box, _p(counts, C.c_int32))
+    rc = _REF_CUB.ref_detect_cuboid_skew(_p(img, C.c_uint8), w, h, ch, _p(K, C.c_double), _p(T_wc, C.c_double), _p(boxes, C.c_double), N,
+                                         _p(lines, C.c_double), len(lines), _p(flags, C.c_int32), C.c_double(params.nominal_skew_ratio),
+                                         C.c_double(params.max_cut_skew), int(params.max_cuboid_num), out.ctypes.data_as(C.POINTER(C.c_double)),
+                                         cap_per_box, _p(counts, C.c_int32))
     if rc != 0:
         raise RuntimeError("ref_detect_cuboid failed (%d)" % rc)
     return [out[b, :min(counts[b], cap_per_box)].copy() for b in range(N)]

@@ -25,8 +25,10 @@ def _oracle_params(O, **kw):
 def _compare_cuboid(g, o, tight=TIGHT):
     assert int(g["proposal_index"]) == int(o["proposal_index"])
     assert int(g["height_sample_id"]) == int(o["height_sample_id"])
-    # NaN on both sides where every proposal of a box has the same errors (the reference's normalisation divides 0 by 0): equal
-    assert abs(float(g["normalized_error"]) - float(o["normalized_error"])) < SCORE_TOL or (np.isnan(g["normalized_error"]) and np.isnan(o["normalized_error"]))
+    # NaN on both sides where every proposal of a box has the same errors (the reference's normalisation divides 0 by 0): equal.
+    # The same infinity on both sides where weight_vp_angle = -1 divides by 1 + w = 0: equal
+    gn, on = float(g["normalized_error"]), float(o["normalized_error"])
+    assert abs(gn - on) < SCORE_TOL or (np.isnan(gn) and np.isnan(on)) or (np.isinf(gn) and gn == on)
     np.testing.assert_allclose(g["normalized_error"], o["normalized_error"], rtol=0, atol=tight)
     np.testing.assert_allclose(g["combined_score"], o["combined_score"], rtol=1e-9, atol=tight)
     np.testing.assert_allclose(g["edge_distance_error"], o["edge_distance_error"], rtol=1e-12, atol=1e-12)
