@@ -59,10 +59,9 @@ struct cs_ctx {
     std::vector<double> yaws;
     std::vector<CsJob> jobs;
     std::vector<CsObj> objs;
-    std::vector<int2> sweep_blocks;
     std::vector<int4> sweep_blocks4; /* warp sweep: (job, pose, first yaw, yaws in block) */
     int max_n_cand = 0;
-    int use_cta_select = 0; /* debug: force the CTA-wide sweep / selection kernels */
+    int use_cta_select = 0; /* debug: force the CTA-wide selection kernel (k_fuse_rank) for every box */
     std::vector<int32_t> dt_ids, tile_job;
     int dt_class_off[CS_DT_CLASSES + 1] = {0}, dt_class_plane_words[CS_DT_CLASSES] = {0};
     int64_t total_px = 0, total_cand = 0, total_bits = 0;
@@ -78,10 +77,10 @@ struct cs_ctx {
     cudaEvent_t ev_mid = nullptr, ev_done = nullptr, ev_dt_fork = nullptr, ev_dt_join = nullptr;
     cudaEvent_t ev_ingest_in = nullptr, ev_ingest_out = nullptr; /* device frames (cs_ingest.cu): producer stream -> context stream -> producer stream */
     int use_prio = 1;
-    int seq_lines = 0;     /* A/B: the plain one-warp-per-frame sequential halves of the line detectors */
+    int seq_lines = 0;     /* A/B: EDLines' round-1 routing and fitting kernels (cs_edlines.cu) */
 
     /* device buffers (grow only) */
-    DevBuf d_img, d_gray, d_lines, d_frames, d_poses, d_yaws, d_jobs, d_objs, d_blocks, d_blocks4, d_dtids, d_tilejob;
+    DevBuf d_img, d_gray, d_lines, d_frames, d_poses, d_yaws, d_jobs, d_objs, d_blocks4, d_dtids, d_tilejob;
     DevBuf d_bits, d_dist, d_mlines, d_lcounts, d_err;
     DevBuf d_cvalid, d_cdist, d_cangle, d_cskew, d_vlist, d_key, d_idx, d_flag, d_keep, d_norm, d_score, d_jcounts;
     DevBuf d_out, d_outcnt, d_gather, d_send;
@@ -200,7 +199,6 @@ int build_tables(cs_ctx *c)
     c->yaws.clear();
     c->jobs.clear();
     c->objs.clear();
-    c->sweep_blocks.clear();
     c->sweep_blocks4.clear();
     c->max_n_cand = 0;
     c->total_px = 0;
@@ -338,7 +336,6 @@ int build_tables(cs_ctx *c)
                 c->n_tiles += jb.tiles_x * ((jb.roi_h + 31) / 32);
                 const int job_id = (int)c->jobs.size();
                 for (int ps = 0; ps < fr.n_pose; ps++) {
-                    c->sweep_blocks.push_back(make_int2(job_id, ps));
                     const int ypb = cs_sweep_warp_yaws();
                     for (int y0 = 0; y0 < fr.n_yaw; y0 += ypb) c->sweep_blocks4.push_back(make_int4(job_id, ps, y0, std::min(ypb, fr.n_yaw - y0)));
                 }
@@ -412,7 +409,6 @@ int prepare_tables(cs_ctx *c)
     if ((rc = upload(c, c->d_yaws, c->yaws))) return rc;
     if ((rc = upload(c, c->d_jobs, c->jobs))) return rc;
     if ((rc = upload(c, c->d_objs, c->objs))) return rc;
-    if ((rc = upload(c, c->d_blocks, c->sweep_blocks))) return rc;
     if ((rc = upload(c, c->d_blocks4, c->sweep_blocks4))) return rc;
     if ((rc = upload(c, c->d_dtids, c->dt_ids))) return rc;
     if ((rc = upload(c, c->d_tilejob, c->tile_job))) return rc;
@@ -481,15 +477,10 @@ int run_batch(cs_ctx *c, bool sync)
     mark(ST_LINES);
     cudaStreamWaitEvent(st, c->ev_join, 0); /* join */
     mark(ST_SWEEP);
-    if (!c->use_cta_select)
-        cs_launch_sweep_warp((const CsJob *)c->d_jobs.p, (const CsFrame *)c->d_frames.p, (const CsPose *)c->d_poses.p, (const double *)c->d_yaws.p,
-                             (const int4 *)c->d_blocks4.p, (int)c->sweep_blocks4.size(), (const double *)c->d_mlines.p, (const int32_t *)c->d_lcounts.p,
-                             (const float *)c->d_dist.p, (uint8_t *)c->d_cvalid.p, (double *)c->d_cdist.p, (double *)c->d_cangle.p, (double *)c->d_cskew.p, &c->prm,
-                             st, &c->launches);
-    else
-        cs_launch_sweep((const CsJob *)c->d_jobs.p, (const CsFrame *)c->d_frames.p, (const CsPose *)c->d_poses.p, (const double *)c->d_yaws.p,
-                        (const int2 *)c->d_blocks.p, (int)c->sweep_blocks.size(), (const double *)c->d_mlines.p, (const int32_t *)c->d_lcounts.p,
-                        (const float *)c->d_dist.p, (uint8_t *)c->d_cvalid.p, (double *)c->d_cdist.p, (double *)c->d_cangle.p, &c->prm, st, &c->launches);
+    cs_launch_sweep_warp((const CsJob *)c->d_jobs.p, (const CsFrame *)c->d_frames.p, (const CsPose *)c->d_poses.p, (const double *)c->d_yaws.p,
+                         (const int4 *)c->d_blocks4.p, (int)c->sweep_blocks4.size(), (const double *)c->d_mlines.p, (const int32_t *)c->d_lcounts.p,
+                         (const float *)c->d_dist.p, (uint8_t *)c->d_cvalid.p, (double *)c->d_cdist.p, (double *)c->d_cangle.p, (double *)c->d_cskew.p, &c->prm,
+                         st, &c->launches);
     mark(ST_FUSE);
     /* the previous batch's all-gather (its own stream) may still be reading the record buffer: only this point has to wait for it */
     if (c->gather_pending) cudaStreamWaitEvent(st, c->ev_gather_done, 0);
@@ -818,7 +809,7 @@ void cs_destroy(cs_ctx *c)
     if (c->edl_state) cs_edl_destroy(c->edl_state);
     if (c->lbd_state) cs_lbd_destroy(c->lbd_state);
     DevBuf *all[] = {&c->d_img,   &c->d_gray,  &c->d_lines,  &c->d_frames, &c->d_poses,   &c->d_yaws, &c->d_jobs, &c->d_objs,
-                     &c->d_blocks, &c->d_blocks4, &c->d_dtids, &c->d_tilejob, &c->d_bits, &c->d_dist, &c->d_mlines, &c->d_lcounts, &c->d_err,
+                     &c->d_blocks4, &c->d_dtids, &c->d_tilejob, &c->d_bits, &c->d_dist, &c->d_mlines, &c->d_lcounts, &c->d_err,
                      &c->d_cvalid, &c->d_cdist, &c->d_cangle, &c->d_cskew, &c->d_vlist,  &c->d_key,     &c->d_idx,  &c->d_flag, &c->d_keep,  &c->d_norm,
                      &c->d_score,  &c->d_jcounts, &c->d_out,  &c->d_outcnt, &c->d_gather, &c->d_send};
     for (DevBuf *b : all)
@@ -1052,9 +1043,9 @@ int cs_set_profiling(cs_ctx *c, int enable)
     c->profiling = (enable & 1) != 0;
     c->use_raster_dt = ((enable & 32) ? 1 : 0) | ((enable & 64) ? 2 : 0); /* bit 5: raster-scan distance transform kernel; bit 6: cone form, bits from global */
     c->use_prio = (enable & 16) == 0;      /* bit 4: keep the whole chain on one stream (no high-priority tail) */
-    c->seq_lines = (enable & 128) != 0;    /* bit 7: sequential seed loop / routing of the line detectors (A/B reference of the speculative kernels) */
+    c->seq_lines = (enable & 128) != 0;    /* bit 7: EDLines' round-1 kernels (routing and fitting on the pixel maps, one thread per frame); LSD does not read it */
     c->use_tma = (enable & 256) == 0;      /* bit 8: the line detectors' tile kernels stage every tile with byte loads (A/B of the TMA path) */
-    c->use_cta_select = (enable & 8) != 0; /* bit 3: CTA-wide sweep / selection kernels (the general path) instead of the warp ones */
+    c->use_cta_select = (enable & 8) != 0; /* bit 3: CTA-wide selection kernel (k_fuse_rank) for every box instead of k_fuse_warp */
     c->carry_cam_pose = (enable & 1024) != 0; /* bit 10: cs_detect_cuboids[_batch] carries the reference's cam_pose from box to box of a sampled frame */
     return CS_OK;
 }

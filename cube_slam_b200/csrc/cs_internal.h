@@ -76,9 +76,9 @@ void cs_lsd_destroy(void *state);           /* called from cs_destroy */
 int cs_lsd_run_device(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int w, int h, int stride, int channels, float line_length_thres, int cap,
                       const float **d_lines, const int32_t **d_counts);
 void cs_ctx_count_launches(cs_ctx *c, int64_t n);
-int cs_ctx_seq_lines(cs_ctx *c);
+int cs_ctx_seq_lines(cs_ctx *c);            /* cs_set_profiling bit 7; read by cs_edlines.cu only */
 int cs_ctx_profiling(cs_ctx *c);            /* cs_set_profiling bit 0 */
-int cs_ctx_use_tma(cs_ctx *c);              /* cs_set_profiling bit 8 clear */            /* cs_set_profiling bit 7 */
+int cs_ctx_use_tma(cs_ctx *c);              /* cs_set_profiling bit 8 clear */
 void **cs_ctx_edl_slot(cs_ctx *c);          /* owned by cs_edlines.cu */
 void cs_edl_destroy(void *state);           /* called from cs_destroy */
 /* EDLines flavour of detect_filter_lines: frames on the device (or host, copied in) -> filtered float32 segments + counts in HBM */

@@ -62,15 +62,12 @@ void cs_launch_roi_lines(const CsJob *d_jobs, int n_jobs, const CsFrame *d_frame
                          const int32_t *d_n_lines_dev, int f32_pitch, double *d_out_lines,
                          int32_t *d_out_counts, int32_t *d_err, double dist_thre, double angle_thre_deg, double len_thre, cudaStream_t st,
                          int64_t *launches);
-void cs_launch_sweep(const CsJob *d_jobs, const CsFrame *d_frames, const CsPose *d_poses, const double *d_yaw, const int2 *d_blocks,
-                     int n_blocks, const double *d_mlines, const int32_t *d_line_counts, const float *d_dist, uint8_t *c_valid, double *c_dist,
-                     double *c_angle, const cs_cuboid_params *prm, cudaStream_t st, int64_t *launches);
 void cs_launch_fuse(const CsObj *d_objs, int n_objs, const CsJob *d_jobs, const CsFrame *d_frames, const CsPose *d_poses, const double *d_yaw,
                     const uint8_t *c_valid, const double *c_dist, const double *c_angle, int32_t *w_vlist, uint64_t *w_key, uint32_t *w_idx,
                     uint8_t *w_flag, int32_t *w_keep, double *w_norm, double *w_score, int32_t *job_counts, cs_cuboid_rec *d_out,
                     int32_t *d_out_counts, int topk, const cs_cuboid_params *prm, cudaStream_t st, int64_t *launches);
 
-void cs_launch_sweep_warp(const CsJob *d_jobs, const CsFrame *d_frames, const CsPose *d_poses, const double *d_yaw, const int4 *d_blocks,
+void cs_launch_sweep_warp(const CsJob *d_jobs, const CsFrame *d_frames, const CsPose *d_poses, const double *d_yaw, const int4 *d_blocks4,
                           int n_blocks, const double *d_mlines, const int32_t *d_line_counts, const float *d_dist, uint8_t *c_valid,
                           double *c_dist, double *c_angle, double *c_skew, const cs_cuboid_params *prm, cudaStream_t st, int64_t *launches);
 void cs_launch_fuse_warp(const CsObj *d_objs, int n_objs, const CsJob *d_jobs, const CsFrame *d_frames, const CsPose *d_poses, const double *d_yaw,

@@ -1,11 +1,12 @@
 /*
  * cs_kernels_sweep.cu -- the proposal sweep, scoring and selection kernels (sm_90a).
  *
- *   k_sweep_score : getVanishingPoints + VP_support_edge_infos + the yaw x top-corner x configuration
- *                   corner chain + box_edge_sum_dists + box_edge_alignment_angle_error
- *                   (box_proposal_detail.cpp:229-465; object_3d_util.cpp:380-492,602-607)
- *   k_fuse_rank   : fuse_normalize_scores_v2 + change_2d_corner_to_3d_object + skew-penalised ranking
- *                   (box_proposal_detail.cpp:472-536; object_3d_util.cpp:495-648)
+ *   k_sweep_warp : getVanishingPoints + VP_support_edge_infos + the yaw x top-corner x configuration
+ *                  corner chain + box_edge_sum_dists + box_edge_alignment_angle_error + skew ratio
+ *                  (box_proposal_detail.cpp:229-465; object_3d_util.cpp:380-492,602-607)
+ *   k_fuse_warp  : fuse_normalize_scores_v2 + change_2d_corner_to_3d_object + skew-penalised ranking, one warp per box
+ *                  (box_proposal_detail.cpp:472-536; object_3d_util.cpp:495-648)
+ *   k_fuse_rank  : the same selection by one CTA per box, for batches with more than cs_fuse_warp_cap() candidates per ROI job
  *
  * FP64 throughout (compiled -fmad=false); the only float32 arithmetic is the dist-map running sum,
  * which the reference also does in float32 and in the same order.
@@ -17,210 +18,6 @@
 #include "cs_geom.cuh"
 #include "cs_internal.h"
 #include "cs_kernels.h"
-
-#define SW_THREADS 256
-#define SW_WARPS (SW_THREADS / 32)
-#define SW_MAX_YC 16
-#define SW_LPL (CS_MAXL_OUT / 32) /* lines per lane */
-
-struct SweepShared {
-    double ang[CS_MAXL_OUT], midx[CS_MAXL_OUT], midy[CS_MAXL_OUT];
-    D2 vps[SW_MAX_YC][3];
-    double vp_angles[SW_MAX_YC][6];
-    D2 corners[SW_THREADS][8];
-    int32_t slot_cand[SW_THREADS];
-    int warp_cnt[SW_WARPS];
-};
-
-/* (value, index) comparators with first-occurrence semantics of Eigen's maxCoeff / minCoeff */
-__device__ __forceinline__ void arg_better_max(double &v, int &i, double ov, int oi)
-{
-    if (oi >= 0 && (i < 0 || ov > v || (ov == v && oi < i))) {
-        v = ov;
-        i = oi;
-    }
-}
-__device__ __forceinline__ void arg_better_min(double &v, int &i, double ov, int oi)
-{
-    if (oi >= 0 && (i < 0 || ov < v || (ov == v && oi < i))) {
-        v = ov;
-        i = oi;
-    }
-}
-
-/* VP_support_edge_infos for one (yaw, vp) by one warp (object_3d_util.cpp:380-425) */
-__device__ __forceinline__ void vp_support_warp(const SweepShared &S, int n_lines, D2 vp, double thre, int vp_id, double *out2)
-{
-    const unsigned FULL = 0xffffffffu;
-    const int lane = threadIdx.x & 31;
-    double raw[SW_LPL];
-    bool inl[SW_LPL];
-    int first = INT_MAX;
-#pragma unroll
-    for (int k = 0; k < SW_LPL; k++) {
-        const int e = lane + 32 * k;
-        inl[k] = false;
-        raw[k] = 0;
-        if (e < n_lines) {
-            raw[k] = cs_pm_atan2(S.midy[e] - vp.y, S.midx[e] - vp.x);
-            const double nrm = g_normalize_to_pi(raw[k]);
-            double d = fabs(S.ang[e] - nrm);
-            d = g_min(d, CS_PI - d);
-            inl[k] = d < thre;
-            if (inl[k] && e < first) first = e;
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) first = min(first, __shfl_xor_sync(FULL, first, o));
-    if (first == INT_MAX) { /* no inlier: NaN (object_3d_util.cpp:383) */
-        if (lane == 0) {
-            out2[0] = nan("");
-            out2[1] = nan("");
-        }
-        return;
-    }
-    /* smooth_jump_angles (object_3d_util.cpp:175-189): base = first inlier's raw angle */
-    const int owner = first & 31, slot = first >> 5;
-    double base = 0;
-#pragma unroll
-    for (int k = 0; k < SW_LPL; k++)
-        if (k == slot) base = raw[k];
-    base = __shfl_sync(FULL, base, owner);
-    double vmax = 0, vmin = 0;
-    int imax = -1, imin = -1;
-#pragma unroll
-    for (int k = 0; k < SW_LPL; k++) {
-        if (inl[k]) {
-            const int e = lane + 32 * k;
-            double v = raw[k];
-            if ((raw[k] - base) < -CS_PI)
-                v = raw[k] + 2 * CS_PI;
-            else if ((raw[k] - base) > CS_PI)
-                v = raw[k] - 2 * CS_PI;
-            arg_better_max(vmax, imax, v, e);
-            arg_better_min(vmin, imin, v, e);
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const double ov = __shfl_xor_sync(FULL, vmax, o);
-        const int oi = __shfl_xor_sync(FULL, imax, o);
-        arg_better_max(vmax, imax, ov, oi);
-        const double pv = __shfl_xor_sync(FULL, vmin, o);
-        const int pi = __shfl_xor_sync(FULL, imin, o);
-        arg_better_min(vmin, imin, pv, pi);
-    }
-    if (lane == 0) {
-        int low = imax, top = imin;
-        if (vp_id > 0) {
-            const int t = low;
-            low = top;
-            top = t;
-        }
-        out2[0] = S.ang[low];
-        out2[1] = S.ang[top];
-    }
-}
-
-extern __shared__ unsigned char sw_smem_raw[];
-
-__global__ void __launch_bounds__(SW_THREADS) k_sweep_score(const CsJob *__restrict__ jobs, const CsFrame *__restrict__ frames,
-                                                            const CsPose *__restrict__ poses, const double *__restrict__ yaw_table,
-                                                            const int2 *__restrict__ blocks /* (job, pose) */,
-                                                            const double *__restrict__ merged_lines, const int32_t *__restrict__ line_counts,
-                                                            const float *__restrict__ dist_arena, uint8_t *__restrict__ c_valid,
-                                                            double *__restrict__ c_dist, double *__restrict__ c_angle, cs_cuboid_params prm)
-{
-    SweepShared &S = *reinterpret_cast<SweepShared *>(sw_smem_raw);
-    const int2 bp = blocks[blockIdx.x];
-    const CsJob jb = jobs[bp.x];
-    const CsFrame fr = frames[jb.frame];
-    const CsPose &pose = poses[fr.pose_off + bp.y];
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int n_lines = line_counts[bp.x * 2 + 1];
-    const int n_yaw = fr.n_yaw, n_top = jb.n_top;
-    const double *yaws = yaw_table + 3 * (size_t)fr.yaw_off; /* {yaw, cos, sin} per entry */
-
-    /* the ROI's merged line set -> shared memory */
-    {
-        const double *ml = merged_lines + (size_t)bp.x * CS_MAXL_OUT * 7;
-        for (int i = tid; i < n_lines; i += SW_THREADS) {
-            S.ang[i] = ml[4 * CS_MAXL_OUT + i];
-            S.midx[i] = ml[5 * CS_MAXL_OUT + i];
-            S.midy[i] = ml[6 * CS_MAXL_OUT + i];
-        }
-    }
-    if (n_top <= 0 || n_yaw <= 0) return;
-    int YC = SW_THREADS / (2 * n_top);
-    YC = max(1, min(YC, SW_MAX_YC));
-    const float *dist = dist_arena + jb.px_off;
-    const int64_t cbase = jb.cand_off + (int64_t)bp.y * n_yaw * n_top * 2;
-    const bool cfg1 = prm.consider_config_1 != 0, cfg2 = prm.consider_config_2 != 0;
-
-    for (int y0 = 0; y0 < n_yaw; y0 += YC) {
-        const int yc = min(YC, n_yaw - y0);
-        __syncthreads();
-        if (tid < yc) g_vanishing_points(pose.KinvR, yaws + 3 * (y0 + tid), S.vps[tid]);
-        __syncthreads();
-        for (int t = wid; t < yc * 3; t += SW_WARPS) {
-            const int yi = t / 3, vp_id = t - yi * 3;
-            const double thre = ((vp_id != 2) ? prm.vp12_edge_angle_thre : prm.vp3_edge_angle_thre) / 180.0 * CS_PI;
-            if (n_lines > 0)
-                vp_support_warp(S, n_lines, S.vps[yi][vp_id], thre, vp_id, &S.vp_angles[yi][vp_id * 2]);
-            else if (lane == 0) {
-                S.vp_angles[yi][vp_id * 2] = nan("");
-                S.vp_angles[yi][vp_id * 2 + 1] = nan("");
-            }
-        }
-        __syncthreads();
-
-        const int n_group = yc * n_top * 2;
-        for (int g0 = 0; g0 < n_group; g0 += SW_THREADS) {
-            const int gi = g0 + tid;
-            bool valid = false;
-            D2 c[8];
-            int yi = 0, config_id = 1;
-            if (gi < n_group) {
-                yi = gi / (n_top * 2);
-                const int r = gi - yi * (n_top * 2);
-                const int ti = r >> 1;
-                config_id = (r & 1) + 1;
-                int vp1pos;
-                if ((config_id == 1) ? cfg1 : cfg2) valid = g_build_corners(jb, S.vps[yi], g_top_x(jb, ti), config_id, prm.shorted_edge_thre, c, vp1pos);
-                c_valid[cbase + (int64_t)y0 * n_top * 2 + gi] = valid ? 1 : 0;
-            }
-            /* ordered compaction of the valid candidates of this stride */
-            const unsigned m = __ballot_sync(0xffffffffu, valid);
-            if (lane == 0) S.warp_cnt[wid] = __popc(m);
-            __syncthreads();
-            int off = 0, total = 0;
-            for (int k = 0; k < SW_WARPS; k++) {
-                if (k < wid) off += S.warp_cnt[k];
-                total += S.warp_cnt[k];
-            }
-            if (valid) {
-                const int slot = off + __popc(m & ((1u << lane) - 1u));
-#pragma unroll
-                for (int k = 0; k < 8; k++) S.corners[slot][k] = c[k];
-                S.slot_cand[slot] = gi;
-            }
-            __syncthreads();
-            /* scoring: one thread per valid proposal, no idle lanes in the low warps */
-            if (tid < total) {
-                const int sg = S.slot_cand[tid];
-                const int syi = sg / (n_top * 2);
-                const int scfg = ((sg - syi * (n_top * 2)) & 1) + 1;
-                const double sum_dist = g_edge_sum_dists(dist, jb.dpitch, jb.roi_w, jb.roi_h, S.corners[tid], (double)jb.roi_l, (double)jb.roi_t, scfg,
-                                                         prm.reweight_edge_distance != 0);
-                const double ang_err = g_angle_error(S.vp_angles[syi], scfg, S.corners[tid]);
-                const int64_t ci = cbase + (int64_t)y0 * n_top * 2 + sg;
-                c_dist[ci] = sum_dist / jb.diag;
-                c_angle[ci] = ang_err;
-            }
-            __syncthreads();
-        }
-    }
-}
 
 /* ------------------------------------------------------------------------------------------ selection */
 #define FU_THREADS 256
@@ -575,9 +372,9 @@ __global__ void __launch_bounds__(FU_THREADS) k_fuse_rank(const CsObj *__restric
 
 
 /* ==========================================================================================
- * Warp-centric variants (the default when they apply).  The batch holds only ~10^5 candidates, so the CTA-wide
- * kernels above spend most of their time at __syncthreads; here one warp owns an independent unit of work and only
- * __syncwarp is used.
+ * Warp-centric kernels: the sweep, and the selection whenever every ROI job fits FW_CAP.  The batch holds only ~10^5
+ * candidates, so a CTA-wide kernel such as k_fuse_rank above spends most of its time at __syncthreads; here one warp owns
+ * an independent unit of work and only __syncwarp is used.
  * ========================================================================================== */
 #define SWW_WARPS 4
 #define SWW_YAWS 4   /* yaws handled by one warp, one after the other */
@@ -1066,17 +863,6 @@ __global__ void __launch_bounds__(32 * FW_WARPS) k_fuse_warp(const CsObj *__rest
 }
 
 /* ------------------------------------------------------------------------------------------ launchers */
-void cs_launch_sweep(const CsJob *d_jobs, const CsFrame *d_frames, const CsPose *d_poses, const double *d_yaw, const int2 *d_blocks,
-                     int n_blocks, const double *d_mlines, const int32_t *d_line_counts, const float *d_dist, uint8_t *c_valid, double *c_dist,
-                     double *c_angle, const cs_cuboid_params *prm, cudaStream_t st, int64_t *launches)
-{
-    if (n_blocks <= 0) return;
-    CS_ONCE_PER_DEVICE(cudaFuncSetAttribute(k_sweep_score, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SweepShared)));
-    k_sweep_score<<<n_blocks, SW_THREADS, sizeof(SweepShared), st>>>(d_jobs, d_frames, d_poses, d_yaw, d_blocks, d_mlines, d_line_counts, d_dist,
-                                                                     c_valid, c_dist, c_angle, *prm);
-    (*launches)++;
-}
-
 void cs_launch_fuse(const CsObj *d_objs, int n_objs, const CsJob *d_jobs, const CsFrame *d_frames, const CsPose *d_poses, const double *d_yaw,
                     const uint8_t *c_valid, const double *c_dist, const double *c_angle, int32_t *w_vlist, uint64_t *w_key, uint32_t *w_idx,
                     uint8_t *w_flag, int32_t *w_keep, double *w_norm, double *w_score, int32_t *job_counts, cs_cuboid_rec *d_out,
@@ -1090,13 +876,13 @@ void cs_launch_fuse(const CsObj *d_objs, int n_objs, const CsJob *d_jobs, const 
     (*launches)++;
 }
 
-void cs_launch_sweep_warp(const CsJob *d_jobs, const CsFrame *d_frames, const CsPose *d_poses, const double *d_yaw, const int4 *d_blocks,
+void cs_launch_sweep_warp(const CsJob *d_jobs, const CsFrame *d_frames, const CsPose *d_poses, const double *d_yaw, const int4 *d_blocks4,
                           int n_blocks, const double *d_mlines, const int32_t *d_line_counts, const float *d_dist, uint8_t *c_valid,
                           double *c_dist, double *c_angle, double *c_skew, const cs_cuboid_params *prm, cudaStream_t st, int64_t *launches)
 {
     if (n_blocks <= 0) return;
     CS_APPLY_CARVEOUT(k_sweep_warp);
-    k_sweep_warp<<<n_blocks, 32 * SWW_WARPS, 0, st>>>(d_jobs, d_frames, d_poses, d_yaw, d_blocks, d_mlines, d_line_counts, d_dist, c_valid, c_dist,
+    k_sweep_warp<<<n_blocks, 32 * SWW_WARPS, 0, st>>>(d_jobs, d_frames, d_poses, d_yaw, d_blocks4, d_mlines, d_line_counts, d_dist, c_valid, c_dist,
                                                       c_angle, c_skew, *prm);
     (*launches)++;
 }

@@ -236,7 +236,7 @@ void *cs_stream(cs_ctx *ctx);
 /* milliseconds spent in the named stage of the last cs_batch_run ("lsd","gray","canny","hyst","dt","lines","sweep","fuse","total") */
 int cs_stage_ms(cs_ctx *ctx, const char *stage, float *ms);
 /* bit 0: per-stage CUDA-event timing (adds event records only; the chain then stays on one stream).  Debug / A-B switches:
- * bit 3 CTA-wide sweep / selection kernels, bit 4 no high-priority
+ * bit 3 CTA-wide selection kernel (k_fuse_rank) for every box, bit 4 no high-priority
  * stream for the distance transform -> sweep -> selection tail, bit 5 raster-scan distance transform (one kernel) instead of the cone form,
  * bit 6 cone-form distance transform reading the edge bits from global memory (the path of ROIs whose bit plane exceeds 96 KB),
  * bit 7 the line detectors' round-1 kernels (EDLines: routing and fitting on the pixel maps, one thread per frame) instead of the walk-graph

@@ -126,10 +126,6 @@ void cs_launch_roi_lines(const CsJob *, int, const CsFrame *, const double *, co
                          cudaStream_t, int64_t *)
 {
 }
-void cs_launch_sweep(const CsJob *, const CsFrame *, const CsPose *, const double *, const int2 *, int, const double *, const int32_t *, const float *, uint8_t *, double *,
-                     double *, const cs_cuboid_params *, cudaStream_t, int64_t *)
-{
-}
 void cs_launch_sweep_warp(const CsJob *, const CsFrame *, const CsPose *, const double *, const int4 *, int, const double *, const int32_t *, const float *, uint8_t *,
                           double *, double *, double *, const cs_cuboid_params *, cudaStream_t, int64_t *)
 {

@@ -170,8 +170,9 @@ def _dense_batches(oracle, kw):
 
 @pytest.mark.parametrize("mode,kw", (("top5", dict(max_cuboid_num=5)), ("height_top5", dict(whether_sample_bbox_height=1, max_cuboid_num=5))))
 def test_dense_line_sets(cs, oracle, mode, kw):
-    """The warp sweep / selection kernels and the CTA-wide ones (bit 3) on ROIs with about 700 lines inside and more than 200 merged, the 500-merge cap and odd lines."""
-    reached_cap = reached_cta = 0
+    """The warp sweep followed by the warp selection kernel and by the CTA-wide one (bit 3) on ROIs with about 700 lines inside and more than 200
+    merged, the 500-merge cap and odd lines."""
+    reached_cap = reached_dense = 0
     for (w, h), (bt, tags) in _dense_batches(oracle, kw).items():
         for f, tag in enumerate(tags):
             img, T, boxes, lines = bt.frames[f]
@@ -179,12 +180,12 @@ def test_dense_line_sets(cs, oracle, mode, kw):
                 l, t, r, b = E.roi_of(boxes[0], w, h)
                 L = lines[[l <= min(x[0], x[2]) and max(x[0], x[2]) <= r and t <= min(x[1], x[3]) and max(x[1], x[3]) <= b for x in lines]]
                 reached_cap += len(L) - len(oracle.merge_break_lines(L, len_thre=0)) == 500
-        reached_cta += any(jb["trace"]["n_lines_merged"] > 64 for jb in bt.jobs)
+        reached_dense += any(jb["trace"]["n_lines_merged"] > 64 for jb in bt.jobs)
         for flags in (0, 8):
             ctx = cs.Context(0, w, h, len(bt.frames), 4, 8192)
             bt.run(cs, ctx, flags)
             ctx.close()
-    assert reached_cap == 2 and reached_cta == 2, (reached_cap, reached_cta)
+    assert reached_cap == 2 and reached_dense == 2, (reached_cap, reached_dense)
 
 
 def test_large_roi_global_hysteresis_and_dt(cs, oracle):

@@ -1,7 +1,7 @@
 """GPU parity of the cuboid stage with every field of cs_cuboid_params off its default: the CUDA path (through the C ABI) against the CPU
 oracle, one table entry per case, each on a small mixed batch -- fixture A, synthetic VGA, KITTI and 1280 x 960 frames with several boxes and
-the lines given (one case detects its lines with the online LSD) -- through the default kernels and through the CTA-wide sweep and selection
-(cs_set_profiling bit 3).
+the lines given (one case detects its lines with the online LSD) -- through the default kernels and through the CTA-wide selection kernel
+k_fuse_rank after the same warp sweep (cs_set_profiling bit 3).
 
 Every record is compared with test_gpu_cuboid_parity's _compare_cuboid, the batch's candidate and valid counts with the oracle's, and for
 one traced ROI per frame Canny, the distance map, the merged lines, the valid set and both error arrays bit for bit.  A field the kernels

@@ -124,7 +124,7 @@ def test_synthetic_batch_matches_oracle(cs, oracle, seed, w, h, kind, nb):
     ctx = cs.Context(0, w, h, F, 16, 4096)
     ctx.set_calibration(K)
     if seed == 11:
-        ctx.L.cs_set_profiling(ctx.h, 8)  # one case through the CTA-wide sweep / selection kernels
+        ctx.L.cs_set_profiling(ctx.h, 8)  # one case through the CTA-wide selection kernel (k_fuse_rank)
     if seed == 13:
         ctx.L.cs_set_profiling(ctx.h, 32)  # one case through the raster-scan distance transform kernel
     p = cs.default_params(max_cuboid_num=3)
