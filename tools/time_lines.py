@@ -61,6 +61,14 @@ def main():
                     " used-map re-checks/frame %.0f, region lists past the shared-memory part (LSD_SEQ_SCAP entries) %d (%.3f %% of seeds grown)") % (
                         pf[3] / 1e6, pf[0] / 1e6, pf[1] / 1e6, pf[2] / 1e6, pf[6] / 1e6, pf[5], pf[7], pf[4], int(prof[8]),
                         100.0 * float(prof[8]) / max(float(prof[4]), 1.0))
+            hist = [int(prof[15]) >> s & ((1 << 21) - 1) for s in (0, 21, 42)]
+            msg += ("\n    outside the growth pass, Mcycles/frame: hand-off (used-word re-read + seed mask) %.2f, density + candidate store %.2f,"
+                    " reduce_region_radius %.2f (with its region2rect), unattributed %.2f"
+                    " | per frame: seeds reaching region2rect %.1f, refines %.1f, reduce iterations %.1f,"
+                    " region2rect sizes <=32 / <=64 / >64: %.1f / %.1f / %.1f") % (
+                        pf[9] / 1e6, pf[10] / 1e6, pf[11] / 1e6,
+                        (pf[6] - pf[3] - pf[0] - pf[1] - pf[2] - pf[10] - pf[11]) / 1e6,
+                        pf[12], pf[13], pf[14], hist[0] / args.frames, hist[1] / args.frames, hist[2] / args.frames)
         print(msg, flush=True)
 
 
