@@ -8,7 +8,7 @@ from . import _lib  # noqa: F401
 from ._lib import CUBOID_DTYPE  # noqa: F401
 from .detect_3d_cuboid import (Context, CubeSlamError, cuboid, cuboid_draw_edges, cuboid_measurement, default_params, detect_3d_cuboid,  # noqa: F401
                                plot_image_with_cuboid)
-from .line_lbd import BinaryDescriptorMatcher, line_lbd_detect  # noqa: F401
+from .line_lbd import BinaryDescriptorMatcher, LSDDetector, line_lbd_detect  # noqa: F401
 
-__all__ = ["BinaryDescriptorMatcher", "Context", "CubeSlamError", "cuboid", "cuboid_draw_edges", "cuboid_measurement", "default_params", "detect_3d_cuboid", "line_lbd_detect",
+__all__ = ["BinaryDescriptorMatcher", "Context", "LSDDetector", "CubeSlamError", "cuboid", "cuboid_draw_edges", "cuboid_measurement", "default_params", "detect_3d_cuboid", "line_lbd_detect",
            "plot_image_with_cuboid"]

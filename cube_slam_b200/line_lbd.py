@@ -6,6 +6,8 @@ detect_descrip_lines_octaves, match_line_descrip; :191-198,224-356) return numpy
 (the KeyLine fields, octave 0), descriptors as n x 32 uint8 (the CV_8UC1 matrix), matches as records of `_lib.DMATCH_DTYPE` (cv::DMatch).
 `line_lbd_detect.bdm` is the class's BinaryDescriptorMatcher (line_lbd_allclass.h:37): pairwise match, knnMatch and radiusMatch on the GPU,
 and the collection forms (add / train / clear, then match / knnMatch / radiusMatch without a train matrix) against codes kept on the GPU.
+`line_lbd_detect.lsd` is the class's LSDDetector (line_lbd_allclass.h:40): detect over the pyrDown pyramid with masks, per octave or flat,
+and over a list of images with one library call per image size.
 detect_filter_lines_device, detect_descrip_lines_device and compute_descriptors_device take frames that are already in GPU memory.
 A detector built with more than one octave (LSD flavour, octaveratio 2) returns every octave from detect_raw_lines_octaves,
 detect_raw_lines and detect_descrip_lines_octaves, key lines as records of `_lib.OCTAVE_KEYLINE_DTYPE`."""
@@ -300,6 +302,127 @@ class BinaryDescriptorMatcher(object):
         return [x for x in lists if len(x) or not compactResult]
 
 
+class LSDDetector(object):
+    """Mirror of cv::line_descriptor::LSDDetector (descriptor.hpp:1004-1067, LSDDetector.cpp:104-287) on the device of `context`: LSD over the
+    pyrDown pyramid, every KeyLine field, as records of `_lib.OCTAVE_KEYLINE_DTYPE` (KeyLine::pt is the mid point of start and end).
+
+    detect(image, scale, numOctaves, mask=None) -> the flat list, octave after octave; detect_octaves(image, scale, numOctaves, mask=None) ->
+    one array per octave; detect([images], scale, numOctaves, masks=None) -> one flat array per image, one library call per (height, width,
+    channels) group.  Images are H x W gray, H x W x 3 BGR or H x W x 4 BGRA, uint8.  numOctaves == 1 ignores scale; numOctaves > 1 needs
+    scale 2 (pyrDown's size rule); numOctaves == 0 detects nothing.  mask: an H x W uint8 array; a key line is dropped when the mask is 0 at
+    both of its truncated end points (LSDDetector.cpp:258-286); class_id keeps counting the lines of an octave before the mask, as in the
+    reference.  A masks list shorter than the images leaves the rest unmasked.  The arrays are new: the C++ overloads' append semantics and
+    LSDOptions do not apply here.  Refusals raise CubeSlamError with the reference's message where it has one."""
+
+    FIRST_CAP = 2048    # LSD segments per octave the first call has room for; doubled while the library answers CS_ERR_CAPACITY
+
+    def __init__(self, context):
+        self._ctx = context
+
+    @staticmethod
+    def _check(img, mask, scale, numOctaves, mask_message):
+        img = np.asarray(img)
+        if mask is not None:
+            m = np.asarray(mask)
+            if m.shape != img.shape[:2] or m.dtype != np.uint8:
+                raise CubeSlamError(mask_message)
+        if img.ndim not in (2, 3) or (img.ndim == 3 and img.shape[2] not in (1, 3, 4)):
+            raise CubeSlamError("LSDDetector takes H x W gray, H x W x 3 BGR or H x W x 4 BGRA images, got shape %s" % (img.shape,))
+        if img.dtype != np.uint8:
+            raise CubeSlamError("Error, depth image!= 0")
+        if numOctaves > 1 and int(scale) != 2:
+            raise CubeSlamError("LSDDetector with more than one octave needs scale 2 (cv::pyrDown makes an octave of (cols / scale, rows / scale) "
+                                "only when |2 * dst - src| <= 2), got %d" % int(scale))
+        if numOctaves < 0:
+            raise CubeSlamError("numOctaves must not be negative (the reference's vector::resize throws std::length_error)")
+
+    @staticmethod
+    def _gray_or_bgr(img):
+        img = np.asarray(img)
+        if img.ndim == 3 and img.shape[2] == 1:
+            return img[..., 0]
+        return img[..., :3] if img.ndim == 3 and img.shape[2] == 4 else img
+
+    @staticmethod
+    def _apply_mask(kl, mask):
+        """LSDDetector.cpp:258-286: drop the lines whose two truncated end points both read 0 (a point outside the mask does not read 0)"""
+        if mask is None or not len(kl):
+            return kl
+        m = np.asarray(mask)
+        H, W = m.shape
+
+        def zero_at(x, y):
+            inside = (x > -1) & (y > -1) & (x < W) & (y < H)
+            xi = np.where(inside, np.trunc(np.where(inside, x, 0)), 0).astype(np.int64)
+            yi = np.where(inside, np.trunc(np.where(inside, y, 0)), 0).astype(np.int64)
+            return inside & (m[yi, xi] == 0)
+        drop = zero_at(kl["start_x"], kl["start_y"]) & zero_at(kl["end_x"], kl["end_y"])
+        return kl[~drop]
+
+    def _detect_group(self, frames, numOctaves):
+        """frames of one size and channel count (F x H x W or F x H x W x 3) -> per frame, one OCTAVE_KEYLINE_DTYPE array per octave"""
+        imgs = np.ascontiguousarray(frames, np.uint8)
+        F, H, W = imgs.shape[:3]
+        ch = 1 if imgs.ndim == 3 else imgs.shape[3]
+        K = int(numOctaves)
+        p = _lib.LineParams()
+        L = self._ctx.L
+        L.cs_default_line_params(C.byref(p))
+        p.use_LSD, p.numoctaves, p.octaveratio = 1, K, 2.0 if K > 1 else 1.0
+        n = np.zeros((F, K), np.int32)
+        cap = self.FIRST_CAP
+        while True:
+            kl = np.zeros((F, K, cap), _lib.OCTAVE_KEYLINE_DTYPE)
+            rc = L.cs_detect_raw_lines_octaves_batch(self._ctx.h, imgs.ctypes.data, F, W, H, W * ch, ch, C.byref(p), kl.ctypes.data, cap,
+                                                     _lib.ptr(n, C.c_int32))
+            if rc == -3 and cap < W * H:        # CS_ERR_CAPACITY: an octave holds more LSD segments than the buffer; twice the room
+                cap *= 2
+                continue
+            self._ctx.check(rc)
+            return [[kl[f, k, :n[f, k]].copy() for k in range(K)] for f in range(F)]
+
+    def _octaves_of(self, images, numOctaves):
+        """one call per (height, width, channels) group -> per image, its octaves"""
+        out = [None] * len(images)
+        if numOctaves < 1:
+            return [[] for _ in images]
+        groups = {}
+        for i, img in enumerate(images):
+            groups.setdefault(img.shape, []).append(i)
+        for idx in groups.values():
+            got = self._detect_group(np.stack([images[i] for i in idx]), numOctaves)
+            for i, g in zip(idx, got):
+                out[i] = g
+        return out
+
+    def _empty(self):
+        return np.zeros(0, _lib.OCTAVE_KEYLINE_DTYPE)
+
+    def detect(self, image, scale, numOctaves, mask=None, masks=None):
+        """detect(image, scale, numOctaves, mask) -> the flat OCTAVE_KEYLINE_DTYPE array; detect([images], scale, numOctaves, masks) -> one
+        per image (the fourth argument is then the list of masks)."""
+        if isinstance(image, (list, tuple)):
+            return self._detect_many(list(image), scale, numOctaves, masks if masks is not None else mask)
+        octs = self.detect_octaves(image, scale, numOctaves, mask)
+        return np.concatenate(octs) if octs else self._empty()
+
+    def detect_octaves(self, image, scale, numOctaves, mask=None):
+        """detect(image, vector<vector<KeyLine>>&, scale, numOctaves, opts, mask) -> one OCTAVE_KEYLINE_DTYPE array per octave"""
+        numOctaves = int(numOctaves)
+        self._check(image, mask, scale, numOctaves, "Mask error while detecting lines: please check its dimensions and that data type is CV_8UC1")
+        octs = self._octaves_of([self._gray_or_bgr(image)], numOctaves)[0]
+        return [self._apply_mask(o, mask) for o in octs]
+
+    def _detect_many(self, images, scale, numOctaves, masks):
+        numOctaves = int(numOctaves)
+        masks = list(masks) if masks is not None else []
+        ms = [masks[i] if i < len(masks) else None for i in range(len(images))]
+        for img, m in zip(images, ms):
+            self._check(img, m, scale, numOctaves, "Masks error while detecting lines: please check their dimensions and that data types are CV_8UC1")
+        found = self._octaves_of([self._gray_or_bgr(x) for x in images], numOctaves)
+        return [self._apply_mask(np.concatenate(o) if o else self._empty(), m) for o, m in zip(found, ms)]
+
+
 class line_lbd_detect(object):
     def __init__(self, numoctaves=1, octaveratio=1.0, device=0, max_width=2048, max_height=2048, context=None):
         self.numoctaves_ = int(numoctaves)
@@ -315,6 +438,14 @@ class line_lbd_detect(object):
         if getattr(self, "_bdm", None) is None:
             self._bdm = BinaryDescriptorMatcher(self._ctx)
         return self._bdm
+
+    @property
+    def lsd(self):
+        """The class's LSDDetector (line_lbd_allclass.h:40), on this detector's context: detect / detect_octaves over the pyrDown pyramid,
+        with masks, and detect([images]) with one library call per image size."""
+        if getattr(self, "_lsd", None) is None:
+            self._lsd = LSDDetector(self._ctx)
+        return self._lsd
 
     def params(self):
         p = _lib.LineParams()
