@@ -345,11 +345,14 @@ struct LsdFrame {
     __device__ __forceinline__ int row_of(int addr) const { return (int)(((unsigned long long)(unsigned)addr * wmagic) >> 40); }
 };
 
-/* the region list of the candidate a warp works on: the first LSD_SEQ_SCAP entries in shared memory (s_seq), the rest in HBM */
+/* the region list of the candidate a warp works on: the first LSD_SEQ_SCAP entries in shared memory (s_seq), the rest in HBM.  Only this
+ * warp writes and reads its entries, so plain loads see the plain stores of put() once a __syncwarp() lies between them; an L2-only load
+ * (__ldcg, a strong GPU-scope load in SASS) there, although it almost never executes, made region2rect and reduce_region_radius, which
+ * read the list at every point, measurably slower (DESIGN.md section 8). */
 struct LsdReg {
     int *g;
     int cap;
-    __device__ __forceinline__ int get(int i) const { return i < LSD_SEQ_SCAP ? s_seq[i] : __ldcg(g + i); }
+    __device__ __forceinline__ int get(int i) const { return i < LSD_SEQ_SCAP ? s_seq[i] : g[i]; }
     __device__ __forceinline__ void put(int i, int v) const
     {
         if (i < LSD_SEQ_SCAP)
