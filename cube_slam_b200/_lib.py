@@ -159,6 +159,9 @@ EXPORTS += LBD_DEVICE_FRAME_EXPORTS
 OCTAVE_EXPORTS = ["cs_detect_raw_lines_octaves_batch", "cs_detect_descrip_lines_octaves_batch", "cs_detect_raw_lines_octaves_batch_device",
                   "cs_detect_descrip_lines_octaves_batch_device"]
 EXPORTS += OCTAVE_EXPORTS
+# descriptors of key lines the caller gives, of any octave (cs_lbd_octaves.cu, cs_ingest.cu), bound the same way
+LBD_OCTAVE_EXPORTS = ["cs_lbd_compute_octaves_batch", "cs_lbd_compute_octaves_batch_device"]
+EXPORTS += LBD_OCTAVE_EXPORTS
 
 
 def load():
@@ -266,9 +269,12 @@ def load():
         L.cs_detect_descrip_lines_octaves_batch.argtypes = [vp, vp, i, i, i, i, i, C.POINTER(LineParams), vp, u8_p, C.c_int32, i32_p]
         L.cs_detect_raw_lines_octaves_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), vp, C.c_int32, i32_p]
         L.cs_detect_descrip_lines_octaves_batch_device.argtypes = [vp, df_p, C.POINTER(LineParams), vp, u8_p, C.c_int32, i32_p]
+    if all(hasattr(L, n) for n in LBD_OCTAVE_EXPORTS):
+        L.cs_lbd_compute_octaves_batch.argtypes = [vp, vp, i, i, i, i, i, vp, i32_p, u8_p, f_p]
+        L.cs_lbd_compute_octaves_batch_device.argtypes = [vp, C.POINTER(DeviceFrames), vp, i32_p, u8_p, f_p]
     for name in EXPORTS:
         if name in (DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS + LSD_DEBUG_EXPORTS + NFA_DEBUG_EXPORTS + LBD_DEVICE_FRAME_EXPORTS
-                    + OCTAVE_EXPORTS) and not hasattr(L, name):
+                    + OCTAVE_EXPORTS + LBD_OCTAVE_EXPORTS) and not hasattr(L, name):
             continue
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("cs_abi_version",):

@@ -327,4 +327,20 @@ int cs_detect_descrip_lines_octaves_batch_device(cs_ctx *c, const cs_device_fram
     return octaves_device(c, frames, params, true, keylines, desc32, max_lines_per_octave, n_lines);
 }
 
+/* cs_lbd_compute_octaves_batch on device frames: the frames go to the EDLines buffer, then the host form's body (cs_lbd_octaves.cu) */
+int cs_lbd_compute_octaves_batch_device(cs_ctx *c, const cs_device_frames *frames, const cs_keyline_octave *keylines, const int32_t *keyline_offsets,
+                                        uint8_t *desc32, float *desc72)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    int rc, n = 0;
+    if ((rc = check_on_ctx(c, frames))) return rc;
+    if ((rc = cs_lbd_octaves_check_given(c, frames->n_frames, frames->width, frames->height, keylines, keyline_offsets, desc32, &n)) || n == 0) return rc;
+    cudaSetDevice(cs_ctx_device(c));
+    const int F = frames->n_frames, W = frames->width, H = frames->height, ch = frames->channels;
+    uint8_t *buf = cs_edl_frame_buffer(c, (size_t)F * H * W * ch);
+    if (!buf) return CS_ERR_CUDA;
+    if ((rc = ingest(c, frames, buf))) return rc;
+    return cs_lbd_compute_octaves_run(c, buf, F, W, H, W * ch, ch, keylines, keyline_offsets, desc32, desc72);
+}
+
 } /* extern "C" */

@@ -163,12 +163,20 @@ void cs_lsd_raw_segments(cs_ctx *c, const float **d_raw, const int32_t **d_nraw)
 /* LSDDetector::detect's KeyLine fill (LSDDetector.cpp:205-250) for one LSD segment `raw` of octave `octave` (an ow x oh image, 2^octave =
  * `scale`) of a w x h input frame: false when the border test drops it (cs_lbd.cu) */
 bool cs_keyline_from_lsd_octave(const float *raw, float scale, int ow, int oh, int w, int h, int octave, int class_id, cs_keyline_octave &o);
-/* the 32-byte descriptors of n key lines, line i of frame frame[i] of the n_frames x h x w Sobel maps d_dx / d_dy, to the host (cs_lbd.cu) */
+/* the 32-byte descriptors of n key lines, line i of frame frame[i] of the n_frames x h x w Sobel maps d_dx / d_dy, to the host, and the
+ * 72-float descriptors when desc72 is not NULL (cs_lbd.cu) */
 int cs_lbd_describe_keylines(cs_ctx *c, const cs_keyline *keylines, const int32_t *frame, int n, const int16_t *d_dx, const int16_t *d_dy, int w,
-                             int h, uint8_t *desc32);
+                             int h, uint8_t *desc32, float *desc72);
 /* the body of the octave calls after their argument checks, on packed frames (rows of `stride` bytes) already on the device */
 int cs_lsd_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width, int height, int stride, int channels, const cs_line_params *params,
                        bool describe, cs_keyline_octave *keylines, uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines);
+/* cs_lbd_compute_octaves_batch's checks of its key lines (the frames are checked by the caller): the CSR, class_id and octave >= 0, every
+ * octave within the pyramid pyrDown can make of a width x height frame; *n the total, 0 = nothing to describe (no output touched) */
+int cs_lbd_octaves_check_given(cs_ctx *c, int n_frames, int width, int height, const cs_keyline_octave *keylines, const int32_t *keyline_offsets,
+                               const uint8_t *desc32, int *n);
+/* its body after the checks, on packed frames (rows of `stride` bytes) already on the device */
+int cs_lbd_compute_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width, int height, int stride, int channels,
+                               const cs_keyline_octave *keylines, const int32_t *keyline_offsets, uint8_t *desc32, float *desc72);
 /* the octave calls' checks of params and max_lines_per_octave (the frames are checked by the caller) */
 int cs_lsd_octaves_check(cs_ctx *c, int width, int height, const cs_line_params *params, const void *keylines, const void *desc32, bool describe,
                          int32_t max_lines_per_octave, const int32_t *n_lines);

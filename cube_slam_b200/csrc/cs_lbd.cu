@@ -329,11 +329,11 @@ bool cs_keyline_from_lsd_octave(const float *raw, float scale, int ow, int oh, i
 }
 
 int cs_lbd_describe_keylines(cs_ctx *c, const cs_keyline *keylines, const int32_t *frame, int n, const int16_t *d_dx, const int16_t *d_dy, int w, int h,
-                             uint8_t *desc32)
+                             uint8_t *desc32, float *desc72)
 {
     std::vector<CsLbdLine> lines((size_t)n);
     for (int i = 0; i < n; i++) lbd_prepare(keylines[i], frame[i], lines[i]);
-    return describe(c, *state_of(c), lines, d_dx, d_dy, w, h, desc32, nullptr);
+    return describe(c, *state_of(c), lines, d_dx, d_dy, w, h, desc32, desc72);
 }
 
 /* ---- shared by the host-frame entry points below and their device-frame forms (cs_ingest.cu) */

@@ -1,9 +1,11 @@
 /* cs_lbd_octaves.cu -- every octave of a multi-octave LSD line_lbd_detect: the image pyramids, LSD per octave, the key lines and their LBD
- * descriptors (include/cube_slam_b200.h: cs_detect_raw_lines_octaves_batch, cs_detect_descrip_lines_octaves_batch).
+ * descriptors (include/cube_slam_b200.h: cs_detect_raw_lines_octaves_batch, cs_detect_descrip_lines_octaves_batch); and the LBD descriptors of
+ * key lines of any octave that the caller gives (cs_lbd_compute_octaves_batch).
  *
  * Replaces   line_lbd/class/line_lbd_allclass.cpp:125-172,285-339   detect_raw_lines (both KeyLine overloads), detect_descrip_lines_octaves
  *            line_lbd/libs/LSDDetector.cpp:55-72,176-250             computeGaussianPyramid, detect: LSD per octave, KeyLine fill
  *            line_lbd/libs/binary_descriptor.cpp:352-398             computeGaussianPyramid + computeSobel for every octave
+ *            line_lbd/libs/binary_descriptor.cpp:587-790             BinaryDescriptor::compute / computeImpl on given key lines of any octave
  *
  *   k_oct_gray      cvtColor of the frames (the fixed-point arithmetic of k_lsd_front / k_ed_front): octave 0 of the LSD pyramid
  *   k_oct_pyrdown   cv::pyrDown on 8-bit planes: the separable 1-4-6-4-1 kernel at the even source positions, BORDER_REFLECT_101, one
@@ -22,9 +24,12 @@
 
 #include <algorithm>
 #include <cmath>
+#include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "cs_internal.h"
+#include "cs_lbd_core.h" /* CS_LBD_BYTES, CS_LBD_DESC */
 
 namespace {
 
@@ -145,6 +150,19 @@ void octave_sizes(int w, int h, int K, std::vector<int> &ow, std::vector<int> &o
     }
 }
 
+/* the descriptor's pyramid (BinaryDescriptor::computeSobel, binary_descriptor.cpp:352-398) of n_frames gray frames: the blurred frame, then
+ * pyrDown per octave into blur (octave k of frame f at off[k] + f * ow[k] * oh[k]); the Sobel maps of octaves k0 .. K - 1 into dx / dy, octave
+ * k at off[k] - off[k0].  2K - k0 launches. */
+void descriptor_pyramid(cudaStream_t st, const uint8_t *gray, int F, const std::vector<int> &ow, const std::vector<int> &oh, const std::vector<size_t> &off,
+                        int K, int k0, uint8_t *blur, int16_t *dx, int16_t *dy)
+{
+    k_oct_blur5<<<grid_for((int64_t)off[1]), 256, 0, st>>>(gray, F, ow[0], oh[0], blur);
+    for (int k = 1; k < K; k++)
+        k_oct_pyrdown<<<grid_for((int64_t)(off[k + 1] - off[k])), 256, 0, st>>>(blur + off[k - 1], F, ow[k - 1], oh[k - 1], blur + off[k], ow[k], oh[k]);
+    for (int k = k0; k < K; k++)
+        k_oct_sobel<<<grid_for((int64_t)(off[k + 1] - off[k])), 256, 0, st>>>(blur + off[k], F, ow[k], oh[k], dx + (off[k] - off[k0]), dy + (off[k] - off[k0]));
+}
+
 }  // namespace
 
 int cs_lsd_octaves_check(cs_ctx *c, int width, int height, const cs_line_params *params, const void *keylines, const void *desc32, bool describe,
@@ -247,12 +265,7 @@ int cs_lsd_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width
             return cs_ctx_fail(c, CS_ERR_CUDA, "cudaMallocAsync(%zu) failed for the descriptor pyramid", off[K] + hi * 4 + 16);
         uint8_t *blur = (uint8_t *)tmp.p;
         int16_t *sob = (int16_t *)(((uintptr_t)(blur + off[K]) + 15) & ~(uintptr_t)15); /* dx of octave k at 2 * (off[k] - off[1]), dy after all dx */
-        k_oct_blur5<<<grid_for((int64_t)off[1]), 256, 0, st>>>(pyr, F, width, height, blur);
-        for (int k = 1; k < K; k++) {
-            k_oct_pyrdown<<<grid_for((int64_t)(off[k + 1] - off[k])), 256, 0, st>>>(blur + off[k - 1], F, ow[k - 1], oh[k - 1], blur + off[k], ow[k], oh[k]);
-            k_oct_sobel<<<grid_for((int64_t)(off[k + 1] - off[k])), 256, 0, st>>>(blur + off[k], F, ow[k], oh[k], sob + (off[k] - off[1]),
-                                                                                 sob + hi + (off[k] - off[1]));
-        }
+        descriptor_pyramid(st, pyr, F, ow, oh, off, K, 1, blur, sob, sob + hi);
         cs_ctx_count_launches(c, 2 * K - 1);
         if (cudaGetLastError() != cudaSuccess)
             return cs_ctx_fail(c, CS_ERR_CUDA, "descriptor pyramid kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -285,7 +298,8 @@ int cs_lsd_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width
                 d_dy = sob + hi + (off[k] - off[1]);
             }
             packed.resize(lines.size() * 32);
-            if ((rc = cs_lbd_describe_keylines(c, lines.data(), frame.data(), (int)lines.size(), d_dx, d_dy, ow[k], oh[k], packed.data()))) return rc;
+            if ((rc = cs_lbd_describe_keylines(c, lines.data(), frame.data(), (int)lines.size(), d_dx, d_dy, ow[k], oh[k], packed.data(), nullptr)))
+                return rc;
             size_t row = 0;
             for (int f = 0; f < F; f++) {
                 const size_t s = (size_t)f * K + k;
@@ -313,6 +327,117 @@ int cs_lsd_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width
             o.kl.class_id = i;
             keylines[s * cap + i] = o;
         }
+    return CS_OK;
+}
+
+/* ---- BinaryDescriptor::compute on key lines the caller gives, of any octave (cs_lbd_compute_octaves_batch[_device]) */
+int cs_lbd_octaves_check_given(cs_ctx *c, int n_frames, int width, int height, const cs_keyline_octave *keylines, const int32_t *keyline_offsets,
+                               const uint8_t *desc32, int *n)
+{
+    *n = 0;
+    if (!keyline_offsets || keyline_offsets[0] != 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "keyline_offsets must start at 0");
+    for (int f = 0; f < n_frames; f++)
+        if (keyline_offsets[f + 1] < keyline_offsets[f]) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "keyline_offsets must not decrease");
+    if (keyline_offsets[n_frames] == 0) return CS_OK; /* "Error: keypoint list is empty": descriptors left as they are (:618-622) */
+    if (!keylines || !desc32) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null key lines or output");
+    /* the deepest octave whose pyramid computeGaussianPyramid can build: pyrDown refuses a level of width or height 0 */
+    int deepest = 0;
+    for (int w = width, h = height; w / 2 > 0 && h / 2 > 0; w /= 2, h /= 2) deepest++;
+    for (int f = 0; f < n_frames; f++)
+        for (int i = keyline_offsets[f]; i < keyline_offsets[f + 1]; i++) {
+            const cs_keyline_octave &o = keylines[i];
+            if (o.kl.class_id < 0 || o.octave < 0)
+                return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "frame %d, row %d: class_id %d and octave %d must not be negative", f, i - keyline_offsets[f],
+                                   o.kl.class_id, o.octave);
+            if (o.octave > deepest)
+                return cs_ctx_fail(c, CS_ERR_INVALID_ARG,
+                                   "frame %d, row %d: octave %d is beyond the pyramid of a %d x %d frame, whose octave %d is %d x %d: pyrDown cannot "
+                                   "make an octave of width or height 0",
+                                   f, i - keyline_offsets[f], o.octave, width, height, deepest, width >> deepest, height >> deepest);
+        }
+    *n = keyline_offsets[n_frames];
+    return CS_OK;
+}
+
+int cs_lbd_compute_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width, int height, int stride, int channels,
+                               const cs_keyline_octave *keylines, const int32_t *keyline_offsets, uint8_t *desc32, float *desc72)
+{
+    cudaSetDevice(cs_ctx_device(c));
+    cudaStream_t st = cs_ctx_stream(c);
+    const int F = n_frames, n = keyline_offsets[F];
+    /* one pyramid as deep as the deepest frame's: the levels a frame does not read do not change its bytes */
+    int K = 0;
+    for (int i = 0; i < n; i++) K = std::max(K, keylines[i].octave + 1);
+    std::vector<int> ow, oh;
+    octave_sizes(width, height, K, ow, oh);
+    std::vector<size_t> off((size_t)K + 1, 0);
+    for (int k = 0; k < K; k++) off[k + 1] = off[k] + (size_t)F * ow[k] * oh[k];
+
+    /* gray frames, the blurred pyramid, and the Sobel maps of every octave (computeSobel(image, max octave + 1), :632-633) */
+    Scratch tmp(st);
+    const size_t bytes = off[1] + off[K] + 16 + off[K] * 4;
+    if (cudaMallocAsync(&tmp.p, bytes, st) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "cudaMallocAsync(%zu) failed for the descriptor pyramid", bytes);
+    uint8_t *gray = (uint8_t *)tmp.p, *blur = gray + off[1];
+    int16_t *dx = (int16_t *)(((uintptr_t)(blur + off[K]) + 15) & ~(uintptr_t)15), *dy = dx + off[K];
+    k_oct_gray<<<grid_for((int64_t)off[1]), 256, 0, st>>>(d_imgs, F, width, height, stride, channels, gray);
+    descriptor_pyramid(st, gray, F, ow, oh, off, K, 0, blur, dx, dy);
+    cs_ctx_count_launches(c, 2 * K + 1);
+    if (cudaGetLastError() != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "descriptor pyramid kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+
+    /* computeLBD per key line on its octave's maps at its in-octave ends (:1207-1250); one launch per octave over every frame */
+    std::vector<cs_keyline> lines;
+    std::vector<int32_t> frame, row;
+    std::vector<uint8_t> packed;
+    std::vector<float> fpacked;
+    for (int k = 0; k < K; k++) {
+        lines.clear();
+        frame.clear();
+        row.clear();
+        for (int f = 0; f < F; f++)
+            for (int i = keyline_offsets[f]; i < keyline_offsets[f + 1]; i++) {
+                const cs_keyline_octave &o = keylines[i];
+                if (o.octave != k) continue;
+                cs_keyline kl = o.kl;
+                kl.start_x = o.s_oct_x;
+                kl.start_y = o.s_oct_y;
+                kl.end_x = o.e_oct_x;
+                kl.end_y = o.e_oct_y;
+                lines.push_back(kl);
+                frame.push_back(f);
+                row.push_back(i);
+            }
+        if (lines.empty()) continue;
+        packed.resize(lines.size() * CS_LBD_BYTES);
+        if (desc72) fpacked.resize(lines.size() * CS_LBD_DESC);
+        int rc;
+        if ((rc = cs_lbd_describe_keylines(c, lines.data(), frame.data(), (int)lines.size(), dx + (off[k] - off[0]), dy + (off[k] - off[0]), ow[k], oh[k],
+                                           packed.data(), desc72 ? fpacked.data() : nullptr)))
+            return rc;
+        for (size_t j = 0; j < row.size(); j++) {
+            memcpy(desc32 + (size_t)row[j] * CS_LBD_BYTES, &packed[j * CS_LBD_BYTES], CS_LBD_BYTES);
+            if (desc72) memcpy(desc72 + (size_t)row[j] * CS_LBD_DESC, &fpacked[j * CS_LBD_DESC], CS_LBD_DESC * sizeof(float));
+        }
+    }
+
+    /* the output map (:655-693, :750-788): the row of a (class_id, octave) pair is the first row that has it, and the rows of the pair are
+     * written there in list order, so it ends with the last one's descriptor; the other rows of the pair keep their own */
+    std::unordered_map<uint64_t, std::pair<int, int>> first_last;
+    for (int f = 0; f < F; f++) {
+        first_last.clear();
+        for (int i = keyline_offsets[f]; i < keyline_offsets[f + 1]; i++) {
+            const uint64_t key = ((uint64_t)(uint32_t)keylines[i].kl.class_id << 32) | (uint32_t)keylines[i].octave;
+            auto it = first_last.emplace(key, std::make_pair(i, i)).first;
+            it->second.second = i;
+        }
+        for (const auto &e : first_last) {
+            const int first = e.second.first, last = e.second.second;
+            if (first == last) continue;
+            memcpy(desc32 + (size_t)first * CS_LBD_BYTES, desc32 + (size_t)last * CS_LBD_BYTES, CS_LBD_BYTES);
+            if (desc72) memcpy(desc72 + (size_t)first * CS_LBD_DESC, desc72 + (size_t)last * CS_LBD_DESC, CS_LBD_DESC * sizeof(float));
+        }
+    }
     return CS_OK;
 }
 
@@ -351,6 +476,24 @@ int cs_detect_descrip_lines_octaves_batch(cs_ctx *c, const uint8_t *imgs, int n_
                                           int32_t *n_lines)
 {
     return octaves_host(c, imgs, n_frames, width, height, stride, channels, params, true, keylines, desc32, max_lines_per_octave, n_lines);
+}
+
+int cs_lbd_compute_octaves_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
+                                 const cs_keyline_octave *keylines, const int32_t *keyline_offsets, uint8_t *desc32, float *desc72)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    if (!imgs || n_frames <= 0 || width <= 0 || height <= 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
+    if (channels != 1 && channels != 3) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "channels must be 1 or 3");
+    if (stride < width * channels) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "stride smaller than a row");
+    int rc, n = 0;
+    if ((rc = cs_lbd_octaves_check_given(c, n_frames, width, height, keylines, keyline_offsets, desc32, &n)) || n == 0) return rc;
+    cudaSetDevice(cs_ctx_device(c));
+    const size_t bytes = (size_t)n_frames * height * stride;
+    uint8_t *buf = cs_edl_frame_buffer(c, bytes);
+    if (!buf) return CS_ERR_CUDA;
+    if (cudaMemcpyAsync(buf, imgs, bytes, cudaMemcpyHostToDevice, cs_ctx_stream(c)) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "H2D copy of frames failed");
+    return cs_lbd_compute_octaves_run(c, buf, n_frames, width, height, stride, channels, keylines, keyline_offsets, desc32, desc72);
 }
 
 }  // extern "C"

@@ -10,7 +10,8 @@ and the collection forms (add / train / clear, then match / knnMatch / radiusMat
 and over a list of images with one library call per image size.
 detect_filter_lines_device, detect_descrip_lines_device and compute_descriptors_device take frames that are already in GPU memory.
 A detector built with more than one octave (LSD flavour, octaveratio 2) returns every octave from detect_raw_lines_octaves,
-detect_raw_lines and detect_descrip_lines_octaves, key lines as records of `_lib.OCTAVE_KEYLINE_DTYPE`."""
+detect_raw_lines and detect_descrip_lines_octaves, key lines as records of `_lib.OCTAVE_KEYLINE_DTYPE`.  compute_descriptors_octaves[_batch|_device]
+describe such key lines, of any octave, that the caller holds -- e.g. what `lsd.detect(img, 2, K)` returned, filtered or reordered."""
 import ctypes as C
 import math
 import numbers
@@ -731,6 +732,51 @@ class line_lbd_detect(object):
         if want_float:
             return [(desc[off[f]:off[f + 1]].copy(), fdesc[off[f]:off[f + 1]].copy()) for f in range(fr.n_frames)]
         return [desc[off[f]:off[f + 1]].copy() for f in range(fr.n_frames)]
+
+    def _octave_keylines(self, keylines_per_frame, n_frames, want_float):
+        """key lines of every frame as one OCTAVE_KEYLINE_DTYPE array, its CSR and the output rows of the octave descriptor calls"""
+        kls = [np.ascontiguousarray(k, _lib.OCTAVE_KEYLINE_DTYPE).reshape(-1) for k in keylines_per_frame]
+        if len(kls) != n_frames:
+            raise CubeSlamError("one key-line array per frame: %d for %d frames" % (len(kls), n_frames))
+        off = np.concatenate([[0], np.cumsum([len(k) for k in kls])]).astype(np.int32)
+        n = int(off[-1])
+        kl = np.ascontiguousarray(np.concatenate(kls)) if n else np.zeros(1, _lib.OCTAVE_KEYLINE_DTYPE)
+        desc = np.zeros((max(n, 1), 32), np.uint8)
+        fdesc = np.zeros((max(n, 1), 72), np.float32) if want_float else None
+        return kl, off, desc, fdesc
+
+    @staticmethod
+    def _rows_per_frame(off, desc, fdesc):
+        F = len(off) - 1
+        if fdesc is not None:
+            return [(desc[off[f]:off[f + 1]].copy(), fdesc[off[f]:off[f + 1]].copy()) for f in range(F)]
+        return [desc[off[f]:off[f + 1]].copy() for f in range(F)]
+
+    def compute_descriptors_octaves(self, gray_img, keylines, want_float=False):
+        """lbd->compute(gray_img, keylines, line_descrips) on key lines of any octave: records of _lib.OCTAVE_KEYLINE_DTYPE, flat and in any
+        order -- e.g. det.lsd.detect(img, 2, K) or a subset of it -> n x 32 uint8 (and the n x 72 float32 descriptor with want_float).  Each
+        key line is described on its own octave of the descriptor's pyramid (max(octave) + 1 levels) from its in-octave ends, angle and
+        numOfPixels.  Rows that share a (class_id, octave) pair follow the reference: the first of them holds the last one's descriptor, the
+        others their own.  A negative class_id or octave, or an octave beyond the pyramid pyrDown can make of the image, raises CubeSlamError."""
+        return self.compute_descriptors_octaves_batch(np.asarray(gray_img)[None], [keylines], want_float)[0]
+
+    def compute_descriptors_octaves_batch(self, imgs, keylines_per_frame, want_float=False):
+        """compute_descriptors_octaves over frames of equal size, frame f with keylines_per_frame[f] (any count including 0, any octaves) ->
+        per frame the n x 32 uint8 descriptors, or (n x 32 uint8, n x 72 float32) with want_float.  One library call for the batch."""
+        imgs, F, H, W, ch = self._frames(imgs)
+        kl, off, desc, fdesc = self._octave_keylines(keylines_per_frame, F, want_float)
+        self._ctx.check(self._ctx.L.cs_lbd_compute_octaves_batch(self._ctx.h, imgs.ctypes.data, F, W, H, W * ch, ch, kl.ctypes.data, _lib.ptr(off, C.c_int32),
+                                                                 _lib.ptr(desc, C.c_uint8), _lib.ptr(fdesc, C.c_float) if want_float else None))
+        return self._rows_per_frame(off, desc, fdesc)
+
+    def compute_descriptors_octaves_device(self, frames, keylines_per_frame, want_float=False, order="bgr", stream=None):
+        """compute_descriptors_octaves_batch on frames already on the GPU (frames, order, stream as detect_filter_lines_device); the same values
+        the host form returns for the same pixels."""
+        fr = _lib.device_frames(frames, order, stream)
+        kl, off, desc, fdesc = self._octave_keylines(keylines_per_frame, fr.n_frames, want_float)
+        self._ctx.check(self._ctx.L.cs_lbd_compute_octaves_batch_device(self._ctx.h, C.byref(fr), kl.ctypes.data, _lib.ptr(off, C.c_int32),
+                                                                        _lib.ptr(desc, C.c_uint8), _lib.ptr(fdesc, C.c_float) if want_float else None))
+        return self._rows_per_frame(off, desc, fdesc)
 
     def get_line_descriptors(self, gray_img, linesmat_src):
         """get_line_descriptors(gray_img, linesmat_src, line_descrips) (:191-198): descriptors of given n x 4 lines.  The reference builds

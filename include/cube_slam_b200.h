@@ -378,6 +378,32 @@ int cs_detect_raw_lines_octaves_batch_device(cs_ctx *ctx, const cs_device_frames
 int cs_detect_descrip_lines_octaves_batch_device(cs_ctx *ctx, const cs_device_frames *frames, const cs_line_params *params,
                                                  cs_keyline_octave *keylines, uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines);
 
+/* BinaryDescriptor::compute(image, keylines, descriptors[, returnFloatDescr]) (binary_descriptor.cpp:587-790, computeSobel :352-398,
+ * computeLBD :1146-1509) on key lines the caller gives, of any octave: the usual line_descriptor pattern of describing what LSDDetector::detect
+ * returned, after the caller kept, reordered or edited it.  One call per frame of the reference, frame f with keylines[keyline_offsets[f] ..
+ * keyline_offsets[f + 1]) in any order:
+ *   - a 3-channel frame is converted to gray (cvtColor BGR2GRAY; the device form follows channel_order);
+ *   - the pyramid has max(octave) + 1 levels: GaussianBlur(5 x 5, sigma 1) of the gray frame, then pyrDown to (cols / 2, rows / 2) per level,
+ *     a 3 x 3 CV_16S Sobel of each -- the descriptor pyramid of cs_detect_descrip_lines_octaves_batch;
+ *   - key line i is described on the maps of its octave, bounded by that octave's width and height, from s_oct_* / e_oct_*, kl.angle and
+ *     kl.num_pixels; kl.start_* / end_* are not read;
+ *   - rows follow the reference's (class_id, octave) map: when several rows share a pair, the first of them gets the descriptor of the last of
+ *     them in list order.  The reference never writes the pair's other rows; here each gets its own descriptor.  The reference also reads the
+ *     first line of every class_id from 0 to the largest (:1482-1490) and crashes on a list that skips one, e.g. a filtered subset of a
+ *     detector's list; here such a list is described row by row like any other.
+ * desc32 has room for keyline_offsets[n_frames] rows of 32 bytes, desc72 (optional) for as many rows of 72 floats.  A frame without key lines
+ * writes nothing (the reference prints "keypoint list is empty" and returns).  Errors, all found before anything is enqueued:
+ * CS_ERR_INVALID_ARG for a negative class_id or octave (undefined in the reference) and for an octave beyond the pyramid pyrDown can make of
+ * the frame (a level of width or height 0, where the reference throws), each naming the frame and the row within it.  Frames of different
+ * depths may share a batch.  C++ code that calls the reference's lbd->compute keeps the reference's (INTEGRATION.md section 2).  Synchronous. */
+int cs_lbd_compute_octaves_batch(cs_ctx *ctx, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
+                                 const cs_keyline_octave *keylines, const int32_t *keyline_offsets /* n_frames + 1 */, uint8_t *desc32,
+                                 float *desc72 /* optional */);
+/* the same on frames already in GPU memory (cs_device_frames); the key lines and their CSR stay host buffers; the frames go to the EDLines
+ * detector's own buffer, as in cs_lbd_compute_batch_device.  Synchronous. */
+int cs_lbd_compute_octaves_batch_device(cs_ctx *ctx, const cs_device_frames *frames, const cs_keyline_octave *keylines,
+                                        const int32_t *keyline_offsets, uint8_t *desc32, float *desc72);
+
 /* line_lbd_detect::match_line_descrip(query, train, good_matches, matching_dist_thres) (line_lbd_allclass.cpp:341-356) over
  * BinaryDescriptorMatcher::match (line_lbd/libs/binary_descriptor_matcher.cpp:196-262): for every query descriptor the train descriptor
  * at the smallest Hamming distance -- of several, the one the reference's multi-index hash meets first -- kept when distance < thres.
