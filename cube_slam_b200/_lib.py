@@ -72,6 +72,25 @@ class DeviceFrames(C.Structure):
 ORDERS = {"bgr": 0, "rgb": 1}   # CS_ORDER_BGR, CS_ORDER_RGB
 
 
+class FrameView(C.Structure):
+    """cs_frame_view: one frame of a batch of frames of different sizes, `offset` bytes from the batch's base pointer."""
+    _fields_ = [("offset", C.c_int64), ("width", C.c_int32), ("height", C.c_int32), ("stride", C.c_int32), ("channels", C.c_int32)]
+
+
+def pack_frames(imgs):
+    """H x W gray or H x W x 3 uint8 images -> (one contiguous byte buffer, FrameView array) for the *_mixed calls"""
+    views = (FrameView * len(imgs))()
+    parts, off = [], 0
+    for i, a in enumerate(imgs):
+        a = np.ascontiguousarray(a, np.uint8)
+        ch = 1 if a.ndim == 2 else a.shape[2]
+        views[i].offset, views[i].height, views[i].width, views[i].channels = off, a.shape[0], a.shape[1], ch
+        views[i].stride = a.shape[1] * ch
+        parts.append(a.reshape(-1))
+        off += a.size
+    return np.concatenate(parts) if parts else np.zeros(0, np.uint8), views
+
+
 def _stream_handle(frames, stream):
     """cudaStream_t the producer wrote `frames` on: the given torch.cuda.Stream or raw handle; else torch's current stream for a torch tensor;
     else the `stream` entry of __cuda_array_interface__ (1: legacy default stream, 2: per-thread default stream); else the legacy default (0)."""
@@ -162,6 +181,9 @@ EXPORTS += OCTAVE_EXPORTS
 # descriptors of key lines the caller gives, of any octave (cs_lbd_octaves.cu, cs_ingest.cu), bound the same way
 LBD_OCTAVE_EXPORTS = ["cs_lbd_compute_octaves_batch", "cs_lbd_compute_octaves_batch_device"]
 EXPORTS += LBD_OCTAVE_EXPORTS
+# batches of frames of different sizes (cs_lsd.cu, cs_lbd_octaves.cu), bound the same way
+MIXED_EXPORTS = ["cs_detect_lines_batch_mixed", "cs_detect_raw_lines_octaves_batch_mixed"]
+EXPORTS += MIXED_EXPORTS
 
 
 def load():
@@ -272,9 +294,13 @@ def load():
     if all(hasattr(L, n) for n in LBD_OCTAVE_EXPORTS):
         L.cs_lbd_compute_octaves_batch.argtypes = [vp, vp, i, i, i, i, i, vp, i32_p, u8_p, f_p]
         L.cs_lbd_compute_octaves_batch_device.argtypes = [vp, C.POINTER(DeviceFrames), vp, i32_p, u8_p, f_p]
+    if all(hasattr(L, n) for n in MIXED_EXPORTS):
+        fv_p = C.POINTER(FrameView)
+        L.cs_detect_lines_batch_mixed.argtypes = [vp, vp, fv_p, i, C.POINTER(LineParams), f_p, C.c_int32, i32_p]
+        L.cs_detect_raw_lines_octaves_batch_mixed.argtypes = [vp, vp, fv_p, i, C.POINTER(LineParams), vp, C.c_int32, i32_p]
     for name in EXPORTS:
         if name in (DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS + LSD_DEBUG_EXPORTS + NFA_DEBUG_EXPORTS + LBD_DEVICE_FRAME_EXPORTS
-                    + OCTAVE_EXPORTS + LBD_OCTAVE_EXPORTS) and not hasattr(L, name):
+                    + OCTAVE_EXPORTS + LBD_OCTAVE_EXPORTS + MIXED_EXPORTS) and not hasattr(L, name):
             continue
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("cs_abi_version",):

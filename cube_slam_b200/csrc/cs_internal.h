@@ -4,6 +4,8 @@
 
 #include <stdint.h>
 
+#include <vector>
+
 #include "../../include/cube_slam_b200.h"
 
 #define CS_MAX_YAW 512        /* yaw samples per object (reference default 16; dense sweep 181) */
@@ -134,9 +136,22 @@ void cs_set_frames_error(const char *msg);  /* what cs_last_error(NULL) reports 
 /* the line detectors' own frame buffers (the ones cs_detect_lines_batch copies host frames into), grown to `bytes`; null on failure */
 uint8_t *cs_lsd_frame_buffer(cs_ctx *c, size_t bytes);
 uint8_t *cs_edl_frame_buffer(cs_ctx *c, size_t bytes);
-/* the body of cs_detect_lines_batch after its argument checks, on host frames or on frames already on the device */
+/* the body of cs_detect_lines_batch after its argument checks, on host frames or on frames already on the device; with views (LSD only), on
+ * frames of different sizes on the device at imgs + views[f].offset; frame_index: the caller's numbers of the frames, for the messages */
 int cs_detect_lines_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int n_frames, int width, int height, int stride, int channels,
-                        const cs_line_params *params, float *lines_xyxy, int32_t max_lines_per_frame, int32_t *n_lines);
+                        const cs_line_params *params, float *lines_xyxy, int32_t max_lines_per_frame, int32_t *n_lines,
+                        const cs_frame_view *views = nullptr, const int32_t *frame_index = nullptr);
+/* ---- batches of frames of different sizes (cs_lsd.cu) */
+/* the host checks of a frame table (cs_detect_lines_batch_mixed's), each failure naming the frame */
+int cs_check_frame_views(cs_ctx *c, const uint8_t *imgs, const cs_frame_view *views, int n_frames);
+/* bytes of the frames packed back to back without row padding, and the copy of host frames into that layout; `packed` their views there */
+size_t cs_packed_frames_bytes(const cs_frame_view *views, int n_frames);
+int cs_pack_host_frames(cs_ctx *c, uint8_t *d_dst, const uint8_t *imgs, const cs_frame_view *views, int n_frames, std::vector<cs_frame_view> &packed);
+/* cs_lsd_run_sync on device frames of different sizes, frame f at d_imgs + views[f].offset: one LSD run over all of them; the raw segments
+ * (cs_lsd_raw_segments) and the filtered ones at cap per frame, in HBM.  cs_debug_lsd and cs_debug_lsd_defb refuse after such a run. */
+#define CS_LSD_MAX_MIXED_FRAMES 33554431 /* frames (or octave planes) of one mixed LSD run: 64 validation CTAs each in a grid's x (2^31 - 1) */
+int cs_lsd_run_mixed_sync(cs_ctx *c, const uint8_t *d_imgs, const cs_frame_view *views, int n_frames, float line_length_thres, int cap,
+                          const float **d_lines, const int32_t **d_counts);
 void cs_lbd_destroy(void *state);           /* called from cs_destroy */
 /* what a synchronous detector run of the descriptor path leaves in HBM: the kept segments and their counts (cap per frame); EDLines: the
  * {direction, numOfPixels} pairs and the Sobel maps the descriptor reads; LSD: the frames the detector read, for the Sobel maps */
@@ -177,8 +192,12 @@ int cs_lbd_octaves_check_given(cs_ctx *c, int n_frames, int width, int height, c
 /* its body after the checks, on packed frames (rows of `stride` bytes) already on the device */
 int cs_lbd_compute_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width, int height, int stride, int channels,
                                const cs_keyline_octave *keylines, const int32_t *keyline_offsets, uint8_t *desc32, float *desc72);
-/* the octave calls' checks of params and max_lines_per_octave (the frames are checked by the caller) */
+/* the octave calls' checks of params and max_lines_per_octave (the frames are checked by the caller); frame >= 0: the frame the size
+ * message names */
 int cs_lsd_octaves_check(cs_ctx *c, int width, int height, const cs_line_params *params, const void *keylines, const void *desc32, bool describe,
-                         int32_t max_lines_per_octave, const int32_t *n_lines);
+                         int32_t max_lines_per_octave, const int32_t *n_lines, int frame = -1);
+/* cs_lsd_octaves_run on frames of any sizes already on the device, frame f at d_imgs + views[f].offset (describe: frames of one size) */
+int cs_lsd_octaves_run_views(cs_ctx *c, const uint8_t *d_imgs, const cs_frame_view *views, int n_frames, const cs_line_params *params, bool describe,
+                             cs_keyline_octave *keylines, uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines);
 
 #endif

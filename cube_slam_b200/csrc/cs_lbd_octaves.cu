@@ -14,9 +14,11 @@
  *                   rounding (sum + 32768) >> 16 -- what k_ed_front computes -- the base of the descriptor's pyramid
  *   k_oct_sobel     3 x 3 Sobel to int16 (BORDER_REFLECT_101) of the descriptor's pyramid, octaves >= 1; octave 0's maps come from
  *                   cs_edl_sobel_maps, as for the one-octave descriptor
- * One thread per output pixel over the whole batch; every plane is a few hundred KB, bound by its bytes.  The LSD of each octave is the
- * one-octave detector (cs_lsd_run_sync) on a gray plane; its raw segments go to the host, where the key lines are filled and filtered
- * (cs_keyline_from_lsd_octave, cs_lbd.cu), and the descriptors are computed per octave by the one-octave descriptor kernel. */
+ *   k_oct_gray_tab / k_oct_pyrdown_tab   the same two on frames of any sizes, one launch per level over every frame (OctPlane table)
+ * One thread per output pixel over the whole batch; every plane is a few hundred KB, bound by its bytes.  LSD runs once over every octave of
+ * every frame (cs_lsd_run_mixed_sync: a batch of planes of different sizes); the raw segments go to the host in one copy, where the key lines
+ * are filled and filtered (cs_keyline_from_lsd_octave, cs_lbd.cu), and the descriptors are computed per octave by the one-octave descriptor
+ * kernel. */
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -80,6 +82,70 @@ __global__ void __launch_bounds__(256) k_oct_pyrdown(const uint8_t *__restrict__
             a += k[j] * t;
         }
         dst[p] = (uint8_t)((a + 128u) >> 8);
+    }
+}
+
+/* One plane of a level of the LSD pyramids of frames of any sizes: its source (sw x sh, rows of sstride bytes, ch channels) and its
+ * destination (dw x dh, packed), and px0, the pixels of the level's earlier planes.  One launch per level covers every frame. */
+struct OctPlane {
+    int64_t src, dst, px0;
+    int32_t sw, sh, sstride, ch, dw, dh, pad_;
+};
+
+/* the plane of the level that output pixel p belongs to: the last one whose px0 is <= p */
+__device__ __forceinline__ int oct_plane_of(const OctPlane *__restrict__ tab, int n, int64_t p)
+{
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (tab[mid].px0 <= p)
+            lo = mid;
+        else
+            hi = mid - 1;
+    }
+    return lo;
+}
+
+/* k_oct_gray over frames of any sizes: octave 0 of every frame's pyramid */
+__global__ void __launch_bounds__(256) k_oct_gray_tab(const uint8_t *__restrict__ img, const OctPlane *__restrict__ tab, int n, int64_t total,
+                                                      uint8_t *__restrict__ pyr)
+{
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < total; p += (int64_t)gridDim.x * blockDim.x) {
+        const OctPlane &P = tab[oct_plane_of(tab, n, p)];
+        const int r = (int)(p - P.px0);
+        const int y = r / P.dw, x = r - y * P.dw;
+        const uint8_t *row = img + P.src + (size_t)y * P.sstride;
+        if (P.ch == 3) {
+            const uint8_t *q = row + 3 * x;
+            pyr[P.dst + r] = (uint8_t)((q[0] * 3735u + q[1] * 19235u + q[2] * 9798u + (1u << 14)) >> 15);
+        } else
+            pyr[P.dst + r] = row[x];
+    }
+}
+
+/* k_oct_pyrdown over frames of any sizes: one level of every frame's pyramid from the level above it, both in pyr */
+__global__ void __launch_bounds__(256) k_oct_pyrdown_tab(const OctPlane *__restrict__ tab, int n, int64_t total, uint8_t *__restrict__ pyr)
+{
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < total; p += (int64_t)gridDim.x * blockDim.x) {
+        const OctPlane &P = tab[oct_plane_of(tab, n, p)];
+        const int r = (int)(p - P.px0);
+        const int y = r / P.dw, x = r - y * P.dw;
+        const uint8_t *s = pyr + P.src;
+        const int sw = P.sw, sh = P.sh;
+        const int k[5] = {1, 4, 6, 4, 1};
+        int xs[5];
+#pragma unroll
+        for (int i = 0; i < 5; i++) xs[i] = oct_reflect101(2 * x + i - 2, sw);
+        uint32_t a = 0;
+#pragma unroll
+        for (int j = 0; j < 5; j++) {
+            const uint8_t *row = s + (size_t)oct_reflect101(2 * y + j - 2, sh) * sw;
+            uint32_t t = 0;
+#pragma unroll
+            for (int i = 0; i < 5; i++) t += k[i] * (uint32_t)row[xs[i]];
+            a += k[j] * t;
+        }
+        pyr[P.dst + r] = (uint8_t)((a + 128u) >> 8);
     }
 }
 
@@ -166,7 +232,7 @@ void descriptor_pyramid(cudaStream_t st, const uint8_t *gray, int F, const std::
 }  // namespace
 
 int cs_lsd_octaves_check(cs_ctx *c, int width, int height, const cs_line_params *params, const void *keylines, const void *desc32, bool describe,
-                         int32_t max_lines_per_octave, const int32_t *n_lines)
+                         int32_t max_lines_per_octave, const int32_t *n_lines, int frame)
 {
     if (!params || !keylines || (describe && !desc32) || !n_lines || max_lines_per_octave <= 0)
         return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
@@ -182,55 +248,103 @@ int cs_lsd_octaves_check(cs_ctx *c, int width, int height, const cs_line_params 
                            (double)params->octaveratio);
     std::vector<int> ow, oh;
     octave_sizes(width, height, K, ow, oh);
-    if (std::lrint(ow[K - 1] * 0.8) < 2 || std::lrint(oh[K - 1] * 0.8) < 2 || width > 32767 || height > 32767)
+    if (std::lrint(ow[K - 1] * 0.8) < 2 || std::lrint(oh[K - 1] * 0.8) < 2 || width > 32767 || height > 32767) {
+        if (frame >= 0)
+            return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "frame %d: octave %d of a %d x %d frame is %d x %d: too small for LSD", frame, K - 1, width, height,
+                               ow[K - 1], oh[K - 1]);
         return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "octave %d of a %d x %d frame is %d x %d: too small for LSD", K - 1, width, height, ow[K - 1], oh[K - 1]);
+    }
     return CS_OK;
 }
 
-int cs_lsd_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width, int height, int stride, int channels, const cs_line_params *params,
-                       bool describe, cs_keyline_octave *keylines, uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines)
+/* the octave calls' body on frames of any sizes on the device, frame f at d_imgs + views[f].offset.  The gray pyramids of every frame, level
+ * after level (K launches); then ONE LSD run over the F x K planes, and the key lines filled on the host from one copy of the raw segments.
+ * describe: frames of one size only (the descriptor's pyramid, descriptor_pyramid, is laid out for one size). */
+int cs_lsd_octaves_run_views(cs_ctx *c, const uint8_t *d_imgs, const cs_frame_view *views, int n_frames, const cs_line_params *params, bool describe,
+                             cs_keyline_octave *keylines, uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines)
 {
     cudaSetDevice(cs_ctx_device(c));
     cudaStream_t st = cs_ctx_stream(c);
     const int F = n_frames, K = params->numoctaves, cap = max_lines_per_octave;
-    std::vector<int> ow, oh;
-    octave_sizes(width, height, K, ow, oh);
-    std::vector<size_t> off((size_t)K + 1, 0); /* plane k of every frame at off[k], frame f at off[k] + f * ow[k] * oh[k] */
-    for (int k = 0; k < K; k++) off[k + 1] = off[k] + (size_t)F * ow[k] * oh[k];
+    if ((int64_t)F * K > CS_LSD_MAX_MIXED_FRAMES) /* before anything is enqueued: LSD runs the F x K planes as one batch */
+        return cs_ctx_fail(c, CS_ERR_CAPACITY, "%d frames x %d octaves: more than the %d planes one LSD run takes", F, K, CS_LSD_MAX_MIXED_FRAMES);
+    /* plane (k, f): octave k of frame f, of size pw x ph, at pyr + poff; planes level after level, frame after frame -- for frames of one size,
+     * octave k of frame f lies at off[k] + f * ow[k] * oh[k], the layout descriptor_pyramid reads */
+    const size_t NP = (size_t)F * K;
+    std::vector<int> pw(NP), ph(NP);
+    std::vector<OctPlane> tab(NP);
+    std::vector<cs_frame_view> planes(NP);
+    std::vector<int64_t> level_px((size_t)K, 0);
+    size_t total = 0;
+    for (int k = 0; k < K; k++)
+        for (int f = 0; f < F; f++) {
+            const size_t q = (size_t)k * F + f, qa = q - F; /* qa: the plane above, octave k - 1 of the same frame */
+            pw[q] = k ? pw[qa] / 2 : views[f].width;    /* Size(cols / scale, rows / scale), scale 2 */
+            ph[q] = k ? ph[qa] / 2 : views[f].height;
+            OctPlane &P = tab[q];
+            memset(&P, 0, sizeof P);
+            P.dst = (int64_t)total;
+            P.dw = pw[q];
+            P.dh = ph[q];
+            P.px0 = level_px[k];
+            if (k == 0) {
+                P.src = views[f].offset;
+                P.sw = views[f].width;
+                P.sh = views[f].height;
+                P.sstride = views[f].stride;
+                P.ch = views[f].channels;
+            } else {
+                P.src = tab[qa].dst;
+                P.sw = pw[qa];
+                P.sh = ph[qa];
+                P.sstride = pw[qa];
+                P.ch = 1;
+            }
+            planes[q].offset = (int64_t)total;
+            planes[q].width = planes[q].stride = pw[q];
+            planes[q].height = ph[q];
+            planes[q].channels = 1;
+            level_px[k] += (int64_t)pw[q] * ph[q];
+            total += (size_t)pw[q] * ph[q];
+        }
 
-    /* the LSD pyramid, in the LSD detector's frame buffer: LSD reads its octaves from there, and cs_debug_lsd of the last octave still can */
-    uint8_t *pyr = cs_lsd_frame_buffer(c, off[K]);
+    /* the LSD pyramids, in the LSD detector's frame buffer (LSD reads its planes from there); their table in scratch until the call ends */
+    uint8_t *pyr = cs_lsd_frame_buffer(c, total);
     if (!pyr) return CS_ERR_CUDA;
-    k_oct_gray<<<grid_for((int64_t)off[1]), 256, 0, st>>>(d_imgs, F, width, height, stride, channels, pyr);
-    for (int k = 1; k < K; k++)
-        k_oct_pyrdown<<<grid_for((int64_t)(off[k + 1] - off[k])), 256, 0, st>>>(pyr + off[k - 1], F, ow[k - 1], oh[k - 1], pyr + off[k], ow[k], oh[k]);
+    Scratch d_tab(st);
+    if (cudaMallocAsync(&d_tab.p, NP * sizeof(OctPlane), st) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "cudaMallocAsync(%zu) failed for the pyramid table", NP * sizeof(OctPlane));
+    if (cudaMemcpyAsync(d_tab.p, tab.data(), NP * sizeof(OctPlane), cudaMemcpyHostToDevice, st) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "upload of the pyramid table failed");
+    const OctPlane *dt = (const OctPlane *)d_tab.p;
+    k_oct_gray_tab<<<grid_for(level_px[0]), 256, 0, st>>>(d_imgs, dt, F, level_px[0], pyr);
+    for (int k = 1; k < K; k++) k_oct_pyrdown_tab<<<grid_for(level_px[k]), 256, 0, st>>>(dt + (size_t)k * F, F, level_px[k], pyr);
     cs_ctx_count_launches(c, K);
     if (cudaGetLastError() != cudaSuccess) return cs_ctx_fail(c, CS_ERR_CUDA, "pyramid kernel launch failed: %s", cudaGetErrorString(cudaGetLastError()));
 
-    /* LSD per octave; the raw segments of each run to the host before the next run overwrites them, then the KeyLine fill */
-    std::vector<cs_keyline_octave> all((size_t)F * K * cap);
-    std::vector<int32_t> cnt((size_t)F * K, 0);
-    std::vector<float> raw((size_t)F * cap * 4);
-    std::vector<int32_t> nraw((size_t)F);
+    /* LSD once over every plane; its raw segments to the host in one copy, then the KeyLine fill, octave after octave */
+    const float *d_lines, *d_raw;
+    const int32_t *d_counts, *d_nraw;
+    int rc;
+    if ((rc = cs_lsd_run_mixed_sync(c, pyr, planes.data(), (int)NP, params->line_length_thres, cap, &d_lines, &d_counts))) return rc;
+    cs_lsd_raw_segments(c, &d_raw, &d_nraw);
+    std::vector<float> raw(NP * cap * 4);
+    std::vector<int32_t> nraw(NP);
+    if (cudaMemcpyAsync(nraw.data(), d_nraw, NP * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaMemcpyAsync(raw.data(), d_raw, raw.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+        return cs_ctx_fail(c, CS_ERR_CUDA, "LSD segment copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+    std::vector<cs_keyline_octave> all(NP * cap);
+    std::vector<int32_t> cnt(NP, 0);
     for (int k = 0; k < K; k++) {
-        const float *d_lines, *d_raw;
-        const int32_t *d_counts, *d_nraw;
-        const uint8_t *d_frames;
-        int rc;
-        if ((rc = cs_lsd_run_sync(c, pyr + off[k], true, F, ow[k], oh[k], ow[k], 1, params->line_length_thres, cap, &d_lines, &d_counts, &d_frames)))
-            return rc;
-        cs_lsd_raw_segments(c, &d_raw, &d_nraw);
-        if (cudaMemcpyAsync(nraw.data(), d_nraw, (size_t)F * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-            cudaMemcpyAsync(raw.data(), d_raw, raw.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
-            return cs_ctx_fail(c, CS_ERR_CUDA, "LSD segment copy failed: %s", cudaGetErrorString(cudaGetLastError()));
         const float scale = (float)(1 << k);
         for (int f = 0; f < F; f++) {
-            if (nraw[f] > cap)
-                return cs_ctx_fail(c, CS_ERR_CAPACITY, "frame %d, octave %d: %d LSD segments exceed max_lines_per_octave = %d", f, k, nraw[f], cap);
+            const size_t q = (size_t)k * F + f;
+            if (nraw[q] > cap)
+                return cs_ctx_fail(c, CS_ERR_CAPACITY, "frame %d, octave %d: %d LSD segments exceed max_lines_per_octave = %d", f, k, nraw[q], cap);
             cs_keyline_octave *o = &all[((size_t)f * K + k) * cap];
             int n = 0;
-            for (int i = 0; i < nraw[f]; i++)
-                if (cs_keyline_from_lsd_octave(&raw[((size_t)f * cap + i) * 4], scale, ow[k], oh[k], width, height, k, n, o[n])) n++;
+            for (int i = 0; i < nraw[q]; i++)
+                if (cs_keyline_from_lsd_octave(&raw[(q * cap + i) * 4], scale, pw[q], ph[q], views[f].width, views[f].height, k, n, o[n])) n++;
             cnt[(size_t)f * K + k] = n;
         }
     }
@@ -241,6 +355,12 @@ int cs_lsd_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width
         }
         return CS_OK;
     }
+
+    const int width = views[0].width, height = views[0].height;
+    std::vector<int> ow, oh;
+    octave_sizes(width, height, K, ow, oh);
+    std::vector<size_t> off((size_t)K + 1, 0); /* plane k of every frame at off[k], frame f at off[k] + f * ow[k] * oh[k] */
+    for (int k = 0; k < K; k++) off[k + 1] = off[k] + (size_t)F * ow[k] * oh[k];
 
     /* detect_descrip_lines_octaves' filter (:312-317): lineLength * (float)pow((float)octaveratio, octave) > line_length_thres */
     size_t n_kept = 0;
@@ -328,6 +448,14 @@ int cs_lsd_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width
             keylines[s * cap + i] = o;
         }
     return CS_OK;
+}
+
+int cs_lsd_octaves_run(cs_ctx *c, const uint8_t *d_imgs, int n_frames, int width, int height, int stride, int channels, const cs_line_params *params,
+                       bool describe, cs_keyline_octave *keylines, uint8_t *desc32, int32_t max_lines_per_octave, int32_t *n_lines)
+{
+    std::vector<cs_frame_view> views((size_t)n_frames);
+    for (int f = 0; f < n_frames; f++) views[f] = cs_frame_view{(int64_t)f * height * stride, width, height, stride, channels};
+    return cs_lsd_octaves_run_views(c, d_imgs, views.data(), n_frames, params, describe, keylines, desc32, max_lines_per_octave, n_lines);
 }
 
 /* ---- BinaryDescriptor::compute on key lines the caller gives, of any octave (cs_lbd_compute_octaves_batch[_device]) */
@@ -476,6 +604,23 @@ int cs_detect_descrip_lines_octaves_batch(cs_ctx *c, const uint8_t *imgs, int n_
                                           int32_t *n_lines)
 {
     return octaves_host(c, imgs, n_frames, width, height, stride, channels, params, true, keylines, desc32, max_lines_per_octave, n_lines);
+}
+
+int cs_detect_raw_lines_octaves_batch_mixed(cs_ctx *c, const uint8_t *imgs, const cs_frame_view *views, int n_frames, const cs_line_params *params,
+                                            cs_keyline_octave *keylines, int32_t max_lines_per_octave, int32_t *n_lines)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    int rc;
+    if ((rc = cs_check_frame_views(c, imgs, views, n_frames))) return rc;
+    for (int f = 0; f < n_frames; f++)
+        if ((rc = cs_lsd_octaves_check(c, views[f].width, views[f].height, params, keylines, nullptr, false, max_lines_per_octave, n_lines, f))) return rc;
+    cudaSetDevice(cs_ctx_device(c));
+    /* the frames go to the EDLines buffer: the LSD buffer takes the pyramids */
+    uint8_t *buf = cs_edl_frame_buffer(c, cs_packed_frames_bytes(views, n_frames));
+    if (!buf) return CS_ERR_CUDA;
+    std::vector<cs_frame_view> packed;
+    if ((rc = cs_pack_host_frames(c, buf, imgs, views, n_frames, packed))) return rc;
+    return cs_lsd_octaves_run_views(c, buf, packed.data(), n_frames, params, false, keylines, nullptr, max_lines_per_octave, n_lines);
 }
 
 int cs_lbd_compute_octaves_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,

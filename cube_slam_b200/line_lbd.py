@@ -462,6 +462,17 @@ class line_lbd_detect(object):
         return self.detect_filter_lines_batch(np.asarray(gray_img)[None], cap)[0]
 
     def detect_filter_lines_batch(self, imgs, cap=4096):
+        """Frames (F x H x W or F x H x W x 3 uint8, or a list of H x W / H x W x 3 images of any sizes) -> per frame n x 4 float32.  A list
+        of differently sized images is one library call (cs_detect_lines_batch_mixed)."""
+        if isinstance(imgs, (list, tuple)) and len({np.shape(x) for x in imgs}) > 1:
+            buf, views = _lib.pack_frames(imgs)
+            F = len(imgs)
+            out = np.zeros((F, cap, 4), np.float32)
+            n = np.zeros(F, np.int32)
+            p = self.params()
+            self._ctx.check(self._ctx.L.cs_detect_lines_batch_mixed(self._ctx.h, buf.ctypes.data, views, F, C.byref(p), _lib.ptr(out, C.c_float), cap,
+                                                                     _lib.ptr(n, C.c_int32)))
+            return [out[f, :n[f]].copy() for f in range(F)]
         imgs = np.ascontiguousarray(imgs, np.uint8)
         if imgs.ndim == 3:
             F, H, W = imgs.shape

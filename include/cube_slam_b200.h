@@ -273,7 +273,25 @@ int cs_detect_lines_batch(cs_ctx *ctx, const uint8_t *imgs, int n_frames, int wi
                           int channels, const cs_line_params *params, float *lines_xyxy, int32_t max_lines_per_frame,
                           int32_t *n_lines /* n_frames */);
 
-/* inspection of the last cs_detect_lines[_batch] run (tests): intermediate images of one frame; any pointer may be NULL */
+/* One frame of a batch of frames of different sizes: `height` rows of `stride` bytes starting `offset` bytes from the batch's base pointer,
+ * each row `width` pixels of `channels` (1 = gray, 3 = BGR) bytes. */
+typedef struct cs_frame_view {
+    int64_t offset;
+    int32_t width, height, stride, channels;
+} cs_frame_view;
+
+/* cs_detect_lines_batch over host frames of different sizes and channel counts: frame f is imgs + views[f].offset; its segments go to
+ * lines_xyxy + f * max_lines_per_frame * 4, n_lines[f] of them -- what cs_detect_lines_batch returns for that frame alone.  LSD runs the
+ * whole list as one batch; EDLines (use_LSD == 0) runs one batch per (width, height, channels) group.  Every argument is checked before
+ * anything is enqueued: null pointers, n_frames <= 0, an empty size, channels other than 1 or 3, stride < width * channels and (LSD) a frame
+ * too small for LSD are CS_ERR_INVALID_ARG naming the frame; more segments than max_lines_per_frame is CS_ERR_CAPACITY naming the frame.
+ * Synchronous. */
+int cs_detect_lines_batch_mixed(cs_ctx *ctx, const uint8_t *imgs, const cs_frame_view *views, int n_frames, const cs_line_params *params,
+                                float *lines_xyxy, int32_t max_lines_per_frame, int32_t *n_lines /* n_frames */);
+
+/* inspection of the last cs_detect_lines[_batch] run (tests): intermediate images of one frame; any pointer may be NULL.  It and
+ * cs_debug_lsd_defb read one-size LSD batches only: after a mixed-size call or an octave call (LSD over planes of several sizes) they return
+ * CS_ERR_UNSUPPORTED. */
 int cs_debug_lsd(cs_ctx *ctx, int frame, int32_t scaled_wh[2], double *scaled, double *modgrad, double *angles, int32_t *list,
                  int32_t *list_len, float *raw_lines, int32_t *n_raw, int cap_raw);
 /* diagnostics of the last LSD run's seed loop: stats4 is kept for ABI stability and reads zero (it described the ordered-speculation kernel
@@ -362,6 +380,12 @@ typedef struct cs_keyline_octave {
 int cs_detect_raw_lines_octaves_batch(cs_ctx *ctx, const uint8_t *imgs, int n_frames, int width, int height, int stride, int channels,
                                       const cs_line_params *params, cs_keyline_octave *keylines, int32_t max_lines_per_octave,
                                       int32_t *n_lines /* n_frames * numoctaves */);
+/* cs_detect_raw_lines_octaves_batch over host frames of different sizes and channel counts (cs_frame_view, as in cs_detect_lines_batch_mixed):
+ * slot (f, k) and n_lines[f * numoctaves + k] hold what cs_detect_raw_lines_octaves_batch returns for frame f alone.  The pyramids of every
+ * frame are built one level per launch, and LSD runs once over every octave of every frame.  The same refusals, naming the frame, and the
+ * frame checks of cs_detect_lines_batch_mixed, all before anything is enqueued; CS_ERR_CAPACITY names the frame and the octave.  Synchronous. */
+int cs_detect_raw_lines_octaves_batch_mixed(cs_ctx *ctx, const uint8_t *imgs, const cs_frame_view *views, int n_frames, const cs_line_params *params,
+                                            cs_keyline_octave *keylines, int32_t max_lines_per_octave, int32_t *n_lines /* n_frames * numoctaves */);
 /* line_lbd_detect::detect_descrip_lines_octaves(gray, keylines_out, line_descrips) (line_lbd_allclass.cpp:285-339) for the same detector:
  * the key lines above whose lineLength * (float)pow(octaveratio, octave) > line_length_thres, with start x <= end x (both pairs of ends
  * swapped and the angle folded into [-pi/2, pi/2] where needed), class_id the position in the octave's kept list, and their 32-byte LBD
