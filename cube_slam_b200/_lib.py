@@ -182,7 +182,8 @@ EXPORTS += OCTAVE_EXPORTS
 LBD_OCTAVE_EXPORTS = ["cs_lbd_compute_octaves_batch", "cs_lbd_compute_octaves_batch_device"]
 EXPORTS += LBD_OCTAVE_EXPORTS
 # batches of frames of different sizes (cs_lsd.cu, cs_lbd_octaves.cu), bound the same way
-MIXED_EXPORTS = ["cs_detect_lines_batch_mixed", "cs_detect_raw_lines_octaves_batch_mixed"]
+MIXED_EXPORTS = ["cs_detect_lines_batch_mixed", "cs_detect_raw_lines_octaves_batch_mixed", "cs_batch_upload_mixed", "cs_batch_upload_online_mixed",
+                 "cs_detect_cuboids_batch_mixed", "cs_detect_frames_batch_mixed"]
 EXPORTS += MIXED_EXPORTS
 
 
@@ -298,6 +299,11 @@ def load():
         fv_p = C.POINTER(FrameView)
         L.cs_detect_lines_batch_mixed.argtypes = [vp, vp, fv_p, i, C.POINTER(LineParams), f_p, C.c_int32, i32_p]
         L.cs_detect_raw_lines_octaves_batch_mixed.argtypes = [vp, vp, fv_p, i, C.POINTER(LineParams), vp, C.c_int32, i32_p]
+        cp_p, lp_p = C.POINTER(CuboidParams), C.POINTER(LineParams)
+        L.cs_batch_upload_mixed.argtypes = [vp, vp, fv_p, i, d_p, d_p, d_p, i32_p, d_p, i32_p, cp_p]
+        L.cs_batch_upload_online_mixed.argtypes = [vp, vp, fv_p, i, d_p, d_p, d_p, i32_p, lp_p, cp_p]
+        L.cs_detect_cuboids_batch_mixed.argtypes = [vp, vp, fv_p, i, d_p, d_p, d_p, i32_p, d_p, i32_p, cp_p, vp, i32_p]
+        L.cs_detect_frames_batch_mixed.argtypes = [vp, vp, fv_p, i, d_p, d_p, d_p, i32_p, lp_p, cp_p, vp, i32_p]
     for name in EXPORTS:
         if name in (DEVICE_FRAME_EXPORTS + MATCHER_EXPORTS + COLLECTION_EXPORTS + LSD_DEBUG_EXPORTS + NFA_DEBUG_EXPORTS + LBD_DEVICE_FRAME_EXPORTS
                     + OCTAVE_EXPORTS + LBD_OCTAVE_EXPORTS + MIXED_EXPORTS) and not hasattr(L, name):

@@ -53,6 +53,8 @@ struct CsJob {
     int32_t tiles_x;
     int32_t bw;                         /* 32-bit words per bit-plane row, ceil(roi_w / 32) */
     int32_t dpitch;                     /* row pitch of the dist map in floats (roi_w rounded up to 4) */
+    int32_t gray_pitch;                 /* row pitch (bytes) of the frame's gray plane */
+    int64_t gray_off;                   /* byte (roi_l, roi_t) of the frame's gray plane, from the batch's frame buffer */
     int64_t bit_off;                    /* offset (words) of this ROI's two bordered bit planes */
     int64_t px_off;                     /* offset (floats) of this ROI's dist map, multiple of 16 */
     int64_t cand_off;                   /* offset into the candidate record arenas */
@@ -144,6 +146,9 @@ int cs_detect_lines_run(cs_ctx *c, const uint8_t *imgs, bool imgs_on_device, int
 /* ---- batches of frames of different sizes (cs_lsd.cu) */
 /* the host checks of a frame table (cs_detect_lines_batch_mixed's), each failure naming the frame */
 int cs_check_frame_views(cs_ctx *c, const uint8_t *imgs, const cs_frame_view *views, int n_frames);
+/* the line detectors' size checks of a frame table (cs_detect_lines_batch_mixed's, each failure naming the frame): LSD's smallest frame and
+ * batch size, EDLines' size bounds, numoctaves >= 1 */
+int cs_check_line_frames(cs_ctx *c, const cs_frame_view *views, int n_frames, const cs_line_params *params);
 /* bytes of the frames packed back to back without row padding, and the copy of host frames into that layout; `packed` their views there */
 size_t cs_packed_frames_bytes(const cs_frame_view *views, int n_frames);
 int cs_pack_host_frames(cs_ctx *c, uint8_t *d_dst, const uint8_t *imgs, const cs_frame_view *views, int n_frames, std::vector<cs_frame_view> &packed);
@@ -152,6 +157,16 @@ int cs_pack_host_frames(cs_ctx *c, uint8_t *d_dst, const uint8_t *imgs, const cs
 #define CS_LSD_MAX_MIXED_FRAMES 33554431 /* frames (or octave planes) of one mixed LSD run: 64 validation CTAs each in a grid's x (2^31 - 1) */
 int cs_lsd_run_mixed_sync(cs_ctx *c, const uint8_t *d_imgs, const cs_frame_view *views, int n_frames, float line_length_thres, int cap,
                           const float **d_lines, const int32_t **d_counts);
+/* the same run enqueued only (the online cuboid batch, cs_mixed.cu): no host sync, no rerun; *d_err is the run's error word, a candidate
+ * overflow shows there */
+int cs_lsd_run_mixed_device(cs_ctx *c, const uint8_t *d_imgs, const cs_frame_view *views, int n_frames, float line_length_thres, int cap,
+                            const float **d_lines, const int32_t **d_counts, const int32_t **d_err);
+/* One plane of a table-driven 8-bit conversion over frames of any sizes: its source (sw x sh, rows of sstride bytes, ch channels) and its
+ * destination (dw x dh, packed), and px0, the pixels of the table's earlier planes (cs_launch_gray_tab, cs_lbd_octaves.cu). */
+struct OctPlane {
+    int64_t src, dst, px0;
+    int32_t sw, sh, sstride, ch, dw, dh, pad_;
+};
 void cs_lbd_destroy(void *state);           /* called from cs_destroy */
 /* what a synchronous detector run of the descriptor path leaves in HBM: the kept segments and their counts (cap per frame); EDLines: the
  * {direction, numOfPixels} pairs and the Sobel maps the descriptor reads; LSD: the frames the detector read, for the Sobel maps */

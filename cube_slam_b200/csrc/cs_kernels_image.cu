@@ -73,7 +73,7 @@ __global__ void __launch_bounds__(256) k_bgr2gray_generic(const uint8_t *__restr
 #define CT 32  /* tile edge */
 #define CTP 64 /* pitch of the staged gray tile in bytes (36 used) */
 
-__global__ void __launch_bounds__(256) k_canny_nms(const uint8_t *__restrict__ gray, int img_w, int img_h, const CsJob *__restrict__ jobs,
+__global__ void __launch_bounds__(256) k_canny_nms(const uint8_t *__restrict__ gray, const CsJob *__restrict__ jobs,
                                                    const int32_t *__restrict__ tile_job, uint32_t *__restrict__ bits_arena, int low, int high)
 {
     /* gray, +2 halo: 36 rows at a pitch of CTP bytes, in two buffers that alternate from tile to tile */
@@ -87,7 +87,8 @@ __global__ void __launch_bounds__(256) k_canny_nms(const uint8_t *__restrict__ g
     const int tile_y = packed & 255;
     const int w = jb.roi_w, h = jb.roi_h, tiles_x = jb.tiles_x;
     const int y0 = tile_y * CT;
-    const uint8_t *src = gray + ((size_t)jb.frame * img_h + jb.roi_t) * img_w + jb.roi_l;
+    const uint8_t *src = gray + jb.gray_off; /* the ROI's top-left byte in its frame's gray plane (frames of a batch may differ in size) */
+    const int pitch = jb.gray_pitch;
     const int tx = threadIdx.x, ty = threadIdx.y;
     const int tid = ty * 32 + tx;
     const int TG22 = 13573; /* (int)(0.4142135623730950488016887242097 * (1 << 15) + 0.5) */
@@ -107,7 +108,7 @@ __global__ void __launch_bounds__(256) k_canny_nms(const uint8_t *__restrict__ g
                 const int ly = i / (CT + 4), lx = i - ly * (CT + 4);
                 const int gy = min(max(y0 + ly - 2, 0), h - 1);
                 const int gx = min(max(x0 + lx - 2, 0), w - 1);
-                pre[q] = __ldg(src + gy * img_w + gx);
+                pre[q] = __ldg(src + gy * pitch + gx);
             }
         }
     };
@@ -882,14 +883,14 @@ void cs_launch_gray(const uint8_t *d_img, uint8_t *d_gray, int n_frames, int w, 
     }
 }
 
-void cs_launch_canny(const uint8_t *d_gray, int img_w, int img_h, const CsJob *d_jobs, int n_jobs, const int32_t *d_tile_job, int n_tiles,
-                     uint32_t *d_bits, size_t bits_bytes, int low, int high, cudaStream_t st, int64_t *launches)
+void cs_launch_canny(const uint8_t *d_base, int, int, const CsJob *d_jobs, int n_jobs, const int32_t *d_tile_job, int n_tiles, uint32_t *d_bits,
+                     size_t bits_bytes, int low, int high, cudaStream_t st, int64_t *launches)
 {
     if (n_jobs <= 0) return;
     cudaMemsetAsync(d_bits, 0, bits_bytes, st); /* zero borders (and stale bits) of every plane */
     if (n_tiles > 0) {
         CS_APPLY_CARVEOUT(k_canny_nms);
-        k_canny_nms<<<n_tiles, dim3(32, 8), 0, st>>>(d_gray, img_w, img_h, d_jobs, d_tile_job, d_bits, low, high);
+        k_canny_nms<<<n_tiles, dim3(32, 8), 0, st>>>(d_base, d_jobs, d_tile_job, d_bits, low, high);
         (*launches)++;
     }
 }

@@ -31,6 +31,7 @@
 #include <vector>
 
 #include "cs_internal.h"
+#include "cs_kernels.h" /* cs_launch_gray_tab */
 #include "cs_lbd_core.h" /* CS_LBD_BYTES, CS_LBD_DESC */
 
 namespace {
@@ -85,12 +86,7 @@ __global__ void __launch_bounds__(256) k_oct_pyrdown(const uint8_t *__restrict__
     }
 }
 
-/* One plane of a level of the LSD pyramids of frames of any sizes: its source (sw x sh, rows of sstride bytes, ch channels) and its
- * destination (dw x dh, packed), and px0, the pixels of the level's earlier planes.  One launch per level covers every frame. */
-struct OctPlane {
-    int64_t src, dst, px0;
-    int32_t sw, sh, sstride, ch, dw, dh, pad_;
-};
+/* One plane of a level of the LSD pyramids of frames of any sizes is an OctPlane (cs_internal.h); one launch per level covers every frame. */
 
 /* the plane of the level that output pixel p belongs to: the last one whose px0 is <= p */
 __device__ __forceinline__ int oct_plane_of(const OctPlane *__restrict__ tab, int n, int64_t p)
@@ -106,7 +102,8 @@ __device__ __forceinline__ int oct_plane_of(const OctPlane *__restrict__ tab, in
     return lo;
 }
 
-/* k_oct_gray over frames of any sizes: octave 0 of every frame's pyramid */
+/* k_oct_gray over frames of any sizes: octave 0 of every frame's pyramid; the gray planes of a cuboid batch of mixed sizes
+ * (cs_launch_gray_tab) */
 __global__ void __launch_bounds__(256) k_oct_gray_tab(const uint8_t *__restrict__ img, const OctPlane *__restrict__ tab, int n, int64_t total,
                                                       uint8_t *__restrict__ pyr)
 {
@@ -230,6 +227,13 @@ void descriptor_pyramid(cudaStream_t st, const uint8_t *gray, int F, const std::
 }
 
 }  // namespace
+
+void cs_launch_gray_tab(const uint8_t *d_img, const OctPlane *d_tab, int n, int64_t total, uint8_t *d_dst, cudaStream_t st, int64_t *launches)
+{
+    if (n <= 0 || total <= 0) return;
+    k_oct_gray_tab<<<grid_for(total), 256, 0, st>>>(d_img, d_tab, n, total, d_dst);
+    (*launches)++;
+}
 
 int cs_lsd_octaves_check(cs_ctx *c, int width, int height, const cs_line_params *params, const void *keylines, const void *desc32, bool describe,
                          int32_t max_lines_per_octave, const int32_t *n_lines, int frame)

@@ -1800,6 +1800,18 @@ int cs_lsd_run_mixed_sync(cs_ctx *c, const uint8_t *d_imgs, const cs_frame_view 
     return CS_OK;
 }
 
+int cs_lsd_run_mixed_device(cs_ctx *c, const uint8_t *d_imgs, const cs_frame_view *views, int n_frames, float line_length_thres, int cap,
+                            const float **d_lines, const int32_t **d_counts, const int32_t **d_err)
+{
+    LsdState *S = state_of(c);
+    const int rc = lsd_run_mixed(c, d_imgs, views, n_frames, line_length_thres, cap, *S);
+    if (rc) return rc;
+    *d_lines = (const float *)S->out.p;
+    *d_counts = (const int32_t *)S->nout.p;
+    *d_err = (const int32_t *)S->err.p;
+    return CS_OK;
+}
+
 int cs_check_frame_views(cs_ctx *c, const uint8_t *imgs, const cs_frame_view *views, int n_frames)
 {
     if (!imgs || !views || n_frames <= 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
@@ -1946,13 +1958,10 @@ int cs_detect_lines_batch(cs_ctx *c, const uint8_t *imgs, int n_frames, int widt
     return cs_detect_lines_run(c, imgs, false, n_frames, width, height, stride, channels, params, lines_xyxy, max_lines_per_frame, n_lines);
 }
 
-int cs_detect_lines_batch_mixed(cs_ctx *c, const uint8_t *imgs, const cs_frame_view *views, int n_frames, const cs_line_params *params,
-                                float *lines_xyxy, int32_t max_lines_per_frame, int32_t *n_lines)
+}
+
+int cs_check_line_frames(cs_ctx *c, const cs_frame_view *views, int n_frames, const cs_line_params *params)
 {
-    if (!c) return CS_ERR_INVALID_ARG;
-    int rc;
-    if ((rc = cs_check_frame_views(c, imgs, views, n_frames))) return rc;
-    if (!params || !lines_xyxy || !n_lines || max_lines_per_frame <= 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
     if (params->use_LSD && n_frames > CS_LSD_MAX_MIXED_FRAMES)
         return cs_ctx_fail(c, CS_ERR_CAPACITY, "%d frames in one LSD batch: at most %d", n_frames, CS_LSD_MAX_MIXED_FRAMES);
     if (params->numoctaves < 1) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "numoctaves must be at least 1");
@@ -1963,6 +1972,19 @@ int cs_detect_lines_batch_mixed(cs_ctx *c, const uint8_t *imgs, const cs_frame_v
         if (!params->use_LSD && (w < 8 || h < 8 || w > 65535 || h > 65535)) /* cs_edl_run's bounds, checked here before any group runs */
             return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "frame %d: a %d x %d image is outside EDLines' sizes (8 .. 65535 per side)", f, w, h);
     }
+    return CS_OK;
+}
+
+extern "C" {
+
+int cs_detect_lines_batch_mixed(cs_ctx *c, const uint8_t *imgs, const cs_frame_view *views, int n_frames, const cs_line_params *params,
+                                float *lines_xyxy, int32_t max_lines_per_frame, int32_t *n_lines)
+{
+    if (!c) return CS_ERR_INVALID_ARG;
+    int rc;
+    if ((rc = cs_check_frame_views(c, imgs, views, n_frames))) return rc;
+    if (!params || !lines_xyxy || !n_lines || max_lines_per_frame <= 0) return cs_ctx_fail(c, CS_ERR_INVALID_ARG, "null or empty argument");
+    if ((rc = cs_check_line_frames(c, views, n_frames, params))) return rc;
     cudaSetDevice(cs_ctx_device(c));
     const size_t slot = (size_t)max_lines_per_frame * 4;
     if (!params->use_LSD) {

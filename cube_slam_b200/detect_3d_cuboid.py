@@ -165,6 +165,48 @@ class Context(object):
         self.check(self.L.cs_batch_upload_online_device(self.h, C.byref(fr), _lib.ptr(Ts, C.c_double), _lib.ptr(boxes, C.c_double),
                                                         _lib.ptr(box_off, C.c_int32), C.byref(line_params), C.byref(params)))
 
+    # -- frames of different sizes and cameras ----------------------------------------------------
+    @staticmethod
+    def _pack_mixed(imgs, Ts, boxes_list, lines_list, K):
+        """imgs: a list of H x W or H x W x 3 uint8 arrays of any sizes; K: None (the context's calibration), one 3 x 3 matrix or F x 3 x 3"""
+        F = len(imgs)
+        buf, views = _lib.pack_frames(imgs)
+        Ts, boxes, box_off, lines, line_off = Context._pack_tables(F, Ts, boxes_list, lines_list)
+        if K is not None:
+            K = np.asarray(K, np.float64)
+            K = np.ascontiguousarray(np.broadcast_to(K.reshape(3, 3), (F, 3, 3)) if K.size == 9 else K.reshape(F, 9)).reshape(F, 9)
+        return buf, views, F, Ts, boxes, box_off, lines, line_off, K
+
+    def _mixed_call(self, name, imgs, Ts, boxes_list, lines_list, line_params, params, K, out):
+        buf, views, F, Ts, boxes, box_off, lines, line_off, K = self._pack_mixed(imgs, Ts, boxes_list, lines_list, K)
+        n_obj, topk = int(box_off[-1]), int(params.max_cuboid_num)
+        Kp = None if K is None else _lib.ptr(K, C.c_double)
+        args = [self.h, buf.ctypes.data, views, F, Kp, _lib.ptr(Ts, C.c_double), _lib.ptr(boxes, C.c_double), _lib.ptr(box_off, C.c_int32)]
+        args += [C.byref(line_params)] if line_params is not None else [_lib.ptr(lines, C.c_double), _lib.ptr(line_off, C.c_int32)]
+        args.append(C.byref(params))
+        if out:
+            rec, counts = np.zeros((max(n_obj, 1), topk), CUBOID_DTYPE), np.zeros(max(n_obj, 1), np.int32)
+            args += [rec.ctypes.data, _lib.ptr(counts, C.c_int32)]
+        self.check(getattr(self.L, name)(*args))
+        self._n_obj, self._topk, self._box_off = n_obj, topk, box_off
+        return (rec[:n_obj], counts[:n_obj]) if out else None
+
+    def upload_mixed(self, imgs, Ts, boxes_list, lines_list, params, K=None):
+        """cs_batch_upload_mixed: upload() over a list of frames of any sizes, each with its own calibration (K: None, 3 x 3 or F x 3 x 3)."""
+        self._mixed_call("cs_batch_upload_mixed", imgs, Ts, boxes_list, lines_list, None, params, K, False)
+
+    def upload_online_mixed(self, imgs, Ts, boxes_list, line_params, params, K=None):
+        """cs_batch_upload_online_mixed: upload_online() over a list of frames of any sizes and calibrations."""
+        self._mixed_call("cs_batch_upload_online_mixed", imgs, Ts, boxes_list, [np.zeros((0, 4))] * len(imgs), line_params, params, K, False)
+
+    def detect_batch_mixed(self, imgs, Ts, boxes_list, lines_list, params, K=None):
+        """cs_detect_cuboids_batch_mixed: detect_batch_host() over a list of frames of any sizes and calibrations -> (records, counts)."""
+        return self._mixed_call("cs_detect_cuboids_batch_mixed", imgs, Ts, boxes_list, lines_list, None, params, K, True)
+
+    def detect_frames_mixed(self, imgs, Ts, boxes_list, line_params, params, K=None):
+        """cs_detect_frames_batch_mixed: detect_frames_host() over a list of frames of any sizes and calibrations -> (records, counts)."""
+        return self._mixed_call("cs_detect_frames_batch_mixed", imgs, Ts, boxes_list, [np.zeros((0, 4))] * len(imgs), line_params, params, K, True)
+
     def detect_frames_host(self, imgs, Ts, boxes_list, line_params, params, out=None, counts=None):
         """cs_detect_frames_batch: detect_filter_lines + detect_cuboid per frame, host buffers in / out."""
         F = len(imgs)

@@ -289,6 +289,32 @@ typedef struct cs_frame_view {
 int cs_detect_lines_batch_mixed(cs_ctx *ctx, const uint8_t *imgs, const cs_frame_view *views, int n_frames, const cs_line_params *params,
                                 float *lines_xyxy, int32_t max_lines_per_frame, int32_t *n_lines /* n_frames */);
 
+/* The cuboid calls over host frames of different sizes, channel counts and cameras: frame f is imgs + views[f].offset (cs_frame_view), with
+ * calibration K + 9 f (K: n_frames x 9 row-major, one per frame; NULL = the context's, cs_set_calibration).  Poses, boxes, lines and their
+ * CSRs are the one-size forms'.  Each frame's records and counts are byte for byte what the one-size call (cs_detect_cuboids_batch,
+ * cs_detect_frames_batch) returns for that frame alone with its K set by cs_set_calibration; records stay in box order.
+ * After either upload, cs_batch_run[_async], cs_batch_fetch, cs_batch_stats_get, cs_batch_device_records, cs_debug_roi / cs_debug_candidates
+ * and cs_allgather_topk work as after the one-size forms.  The frames are packed into the context's buffer (rows without padding); a 3-channel
+ * frame's gray plane is made by one table-driven launch over every such frame, a gray frame is read in place.  Online: LSD runs the whole list
+ * as one batch (a candidate-buffer overflow fails the batch at fetch with CS_ERR_CAPACITY, as in the one-size online batch; cs_debug_lsd
+ * refuses afterwards), EDLines one batch per (width, height, channels) group.  cs_detect_cuboids_batch_mixed honours cs_set_profiling bit 10.
+ * Refused on the host before anything is enqueued, naming the frame: the frame checks of cs_detect_lines_batch_mixed (CS_ERR_INVALID_ARG); a
+ * frame larger than cs_create's max_width x max_height (CS_ERR_CAPACITY); a K entry that is not finite or a K of zero determinant
+ * (CS_ERR_INVALID_ARG); and online, a frame outside the detector's sizes, with cs_detect_lines_batch_mixed's messages.  K == NULL without
+ * cs_set_calibration is CS_ERR_INVALID_ARG.  The uploads wait for the context stream as cs_batch_upload does; the detect calls are
+ * synchronous. */
+int cs_batch_upload_mixed(cs_ctx *ctx, const uint8_t *imgs, const cs_frame_view *views, int n_frames, const double *K, const double *T_wc,
+                          const double *boxes, const int32_t *box_offsets, const double *lines, const int32_t *line_offsets,
+                          const cs_cuboid_params *params);
+int cs_batch_upload_online_mixed(cs_ctx *ctx, const uint8_t *imgs, const cs_frame_view *views, int n_frames, const double *K, const double *T_wc,
+                                 const double *boxes, const int32_t *box_offsets, const cs_line_params *line_params, const cs_cuboid_params *params);
+int cs_detect_cuboids_batch_mixed(cs_ctx *ctx, const uint8_t *imgs, const cs_frame_view *views, int n_frames, const double *K, const double *T_wc,
+                                  const double *boxes, const int32_t *box_offsets, const double *lines, const int32_t *line_offsets,
+                                  const cs_cuboid_params *params, cs_cuboid_rec *out, int32_t *out_counts);
+int cs_detect_frames_batch_mixed(cs_ctx *ctx, const uint8_t *imgs, const cs_frame_view *views, int n_frames, const double *K, const double *T_wc,
+                                 const double *boxes, const int32_t *box_offsets, const cs_line_params *line_params, const cs_cuboid_params *params,
+                                 cs_cuboid_rec *out, int32_t *out_counts);
+
 /* inspection of the last cs_detect_lines[_batch] run (tests): intermediate images of one frame; any pointer may be NULL.  It and
  * cs_debug_lsd_defb read one-size LSD batches only: after a mixed-size call or an octave call (LSD over planes of several sizes) they return
  * CS_ERR_UNSUPPORTED. */
